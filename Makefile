@@ -1,10 +1,10 @@
-# Top-level build: the product library (CUDA, sm_100a only) and the CPU checkers.
+# Top-level build: the product library (CUDA, sm_90a only) and the CPU checkers.
 #
 #   make            -> yadcc_b200/libydsched.so + oracle/libydoracle.so (+ oracle/_ref if /root/reference exists)
 #   make cuda       -> yadcc_b200/libydsched.so
 #   make oracle     -> the checkers
 NVCC ?= /usr/local/cuda/bin/nvcc
-ARCH = -gencode arch=compute_100a,code=sm_100a
+ARCH = -gencode arch=compute_90a,code=sm_90a
 NVCCFLAGS = -O3 -std=c++17 -lineinfo $(ARCH) -Xcompiler -fPIC,-Wall,-Wno-unused-function -Iinclude -Iyadcc_b200/csrc
 CSRC = yadcc_b200/csrc
 LIB = yadcc_b200/libydsched.so

@@ -17,11 +17,11 @@ the previous step's grants are freed (so every step starts from the same servant
           TaskDispatcher (oracle/_ref, compiled verbatim; else the CPU restatement) on the same
           queue -- the whole queue for the 100 k configs, a stated prefix for the bigger ones --
           statuses, servant indices and task ids; a mismatch exits non-zero.
-  roofline  `frac` = DRAM bytes per solve MEASURED with ncu (profiles/r2_dram_traffic.json, the
-          warm figure: caches as the timed loop leaves them) / the CUDA-event time / the measured
-          HBM copy peak.  `model_frac` = SURVEY 8(d)'s matrix-row model (36*S + 32 B per decision:
-          what the reference's O(S)-per-decision scan touches; this solver is O(1) per decision,
-          so the model over-counts by design).  `launch_bound` says what the limiter really is.
+  roofline  `frac` = the compulsory bytes of one solve (requests in, grants + leases out, slot
+          records, servant table) / the CUDA-event time / the HBM peak.  `model_frac` = SURVEY 8(d)'s
+          matrix-row model (36*S + 32 B per decision: what the reference's O(S)-per-decision scan
+          touches; this solver is O(1) per decision, so the model over-counts by design).
+          `launch_bound` says what the limiter really is.
   workloads   sub-records for the other BASELINE configs (cfg2-random, cfg-self, cfg3, cfg4 =
           bloom + dedupe + solve, cfg5 on one GPU), each with value, e2e, cpu_baseline, parity.
   cpu_baseline  the reference's TaskDispatcher on a bounded sample of the same queue, one thread
@@ -143,21 +143,7 @@ def measured_hbm_peak() -> tuple[float, str]:
             return float(json.loads(p.read_text())["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def ncu_traffic(name: str) -> dict | None:
-    """DRAM bytes per solve from the committed ncu captures (profiles/r2_dram_traffic.json)."""
-    try:
-        for f in ("r2f_dram_traffic.json", "r2_dram_traffic.json"):  # (r2f: the fused front kernel; r2: the 13-kernel pipeline)
-            p = ROOT / "profiles" / f
-            if p.exists():
-                rec = json.loads(p.read_text())["workloads"].get(name)
-                if rec:
-                    return rec
-        return None
-    except Exception:
-        return None
+    return 3350.0, "data sheet (H100 SXM HBM3, 3.35 TB/s)"
 
 
 # ---------------------------------------------------------------------------------------------
@@ -266,7 +252,7 @@ def measure_workload(name: str, dev_index: int, steps: int, warmup: int, solver:
 
     w = build_workload(name)
     d = TaskDispatcher(device=dev_index, solver=solver)
-    assert d.backend == "cuda-sm100a"
+    assert d.backend == "cuda-sm90a"
     w.register(d, now=0.0, expires_in=3600.0)
     src = w.build_requests(d)
     stages = Cfg4Stages(d, w, len(src)) if name == "cfg4" else None
@@ -354,9 +340,8 @@ def measure_workload(name: str, dev_index: int, steps: int, warmup: int, solver:
             solver_used = st["solver"]
         if use_packed and n <= 2_000_000:
             # -- timed (e2e, 24-byte requests / 16-byte grants): the plain call, for comparison -----------------
-            # (not for the 10 M queue: as the sixth workload of one process this third pass measured 24.5 ms where the
-            # same call takes 8.4-8.6 ms by the library's own host clock and alone in a fresh process --
-            # profiles/r2f_cfg5_plain_call_diagnostics.log; a harness artefact, not traced further)
+            # (not for the 10 M queue: as the sixth workload of one process this third pass timed several times
+            # slower than the same call alone in a fresh process; a harness artefact, not traced further)
             d.free_tasks(prev_ids)
             d.on_expiration_timer(now=now)
             flush.fill_((it + 7) & 0xFF)
@@ -383,6 +368,7 @@ def measure_workload(name: str, dev_index: int, steps: int, warmup: int, solver:
         ok = g["status"] == STATUS_GRANTED
         prev_ids = g["task_id"][ok].copy()
         assert int(ok.sum()) == granted
+        last_grants = g.copy()
         if it >= warmup:
             # CUDA events on the solve stream (cfg4: the filter stages' kernels + compaction are in prep_ms, the uploads
             # of keys / digests / queue are not: `value` counts from "inputs resident in HBM")
@@ -416,8 +402,26 @@ def measure_workload(name: str, dev_index: int, steps: int, warmup: int, solver:
                                "h2d_bytes_per_step": int(h2d24), "d2h_bytes_per_step": int(d2h24),
                                "call": "yd_wait_for_starting_new_tasks (24-byte requests, 16-byte grants)"}
     extra = {"e2e_ms": e2e_ms, "dev_ms": dev_ms, "launches": launches, "n_solves": n_solves, "wall": wall,
-             "S": S_count, "n": n, "w": w}
+             "S": S_count, "n": n, "w": w, "last_grants": last_grants}
     return rec, extra
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir: str, grants: np.ndarray) -> None:
+    """The grants of the last timed step as float64 arrays, one file per field.  Above DUMP_LIMIT_BYTES a fixed
+    seeded sample of the grants is written instead, with its indices into the batch (sample_index.npy)."""
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    fields = ("status", "servant_index", "task_id")
+    idx = np.arange(len(grants))
+    if len(grants) * 8 * (len(fields) + 1) > DUMP_LIMIT_BYTES:
+        keep = DUMP_LIMIT_BYTES // (8 * (len(fields) + 1))
+        idx = np.sort(np.random.default_rng(0).choice(len(grants), size=keep, replace=False))
+        np.save(d / "sample_index.npy", idx.astype(np.float64))
+    for f in fields:
+        np.save(d / f"grants_{f}.npy", grants[f][idx].astype(np.float64))  # (task ids stay below 2**53)
 
 
 def latency_sweep(dev_index: int, sizes=(1, 32, 1024), reps=200):
@@ -500,11 +504,13 @@ def run_ours(args):
 
         return run_sharded(args, rank, world, local)
 
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > the H100's 50 MB L2
     sampler = ClockSampler(local)
     rec, ex = measure_workload(args.workload, local, args.steps, args.warmup, args.solver, not args.no_cpu_baseline, flush, sampler)
     sampler.stop_flag.set()
     sampler.join(timeout=2)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, ex["last_grants"])
     if rec["parity_in_run"] is False:
         print(json.dumps({"error": "parity_in_run failed", "workload": args.workload}), file=sys.stderr)
 
@@ -523,12 +529,6 @@ def run_ours(args):
     # (16 B), the kept slot order's records (8 B per slot), one servant-table read
     slots = int(sum(min(sv.num_processors, sv.max_tasks) for sv in ex["w"].servants))
     compulsory = 24 * n + 16 * n + 16 * rec["granted_per_step"] + 8 * slots + 36 * S_count
-    tr = ncu_traffic(args.workload)
-    warm = tr.get("warm_bytes") if tr else None
-    cold = tr.get("cold_bytes") if tr else None
-    # what the timed loop really moves lies between the two: L2 is flushed between steps, so inputs come from DRAM
-    # once and intermediates stay in L2; `frac` uses the COLD figure (an upper bound on the traffic)
-    measured = cold if cold is not None else warm
     e2e_ms = ex["e2e_ms"]
     line = {
         "metric": METRIC, "value": rec["value"], "unit": UNIT, "n_gpus": 1, "steps": args.steps, "warmup": args.warmup,
@@ -544,24 +544,19 @@ def run_ours(args):
         "parity_in_run": rec["parity_in_run"],
         "roofline": {
             "bound": "hbm",
-            "kernel": ("k_fused_front (fused.cuh): the whole solve as ONE persistent launch, 148 blocks x 1024 threads, two grid barriers"
+            "kernel": ("k_fused_front (fused.cuh): the whole solve as ONE persistent launch, one 1024-thread block per SM, two grid barriers"
                        if rec["gpu_launches_per_step"] == 1 else
                        f"{rec['solver']} solve pipeline (one CUDA graph, {rec['gpu_launches_per_step']} kernels)"),
             # achieved = ALGORITHMIC (compulsory) bytes per launch / the launch's duration, CUDA events on the solve stream
             "achieved": compulsory / (ms_step / 1e3) / 1e9, "peak": peak, "unit": "GB/s",
             "frac": compulsory / (ms_step / 1e3) / 1e9 / peak,
-            "traffic_frac": (measured / (ms_step / 1e3) / 1e9 / peak) if measured else None,
-            "traffic": cold, "traffic_warm": warm,
-            "traffic_source": (tr or {}).get("source", "no ncu capture committed for this workload"),
             "peak_source": peak_src, "kernel_ms_per_step": ms_step,
             "model_frac": n * model_bytes / (ms_step / 1e3) / 1e9 / peak, "algorithmic_bytes_per_decision_model": model_bytes,
             "compulsory": {"bytes_per_step": compulsory, "frac": compulsory / (ms_step / 1e3) / 1e9 / peak},
-            "launch_bound": {"kernels": rec["gpu_launches_per_step"],
-                             "sum_kernel_us": (tr or {}).get("sum_kernel_us"), "graph_us": 1e3 * ms_step},
+            "launch_bound": {"kernels": rec["gpu_launches_per_step"], "graph_us": 1e3 * ms_step},
             "note": "achieved/frac = compulsory bytes of one solve (requests in, grants + leases out, slot records, servant "
-                    "table: `compulsory`) / CUDA-event time of the launch / measured HBM peak; traffic = ncu dram__bytes "
-                    "read+write of the same launch started cold (traffic_warm: caches as the previous solve left them), "
-                    "traffic_frac the same ratio on it. model_frac is SURVEY 8(d)'s 36*S+32 B per decision (the reference's "
+                    "table: `compulsory`) / CUDA-event time of the launch / HBM peak. "
+                    "model_frac is SURVEY 8(d)'s 36*S+32 B per decision (the reference's "
                     "O(S) scan per decision; this solver does O(1) work per decision, so it exceeds 1). The solve is bound by "
                     "the dependent-latency chain of its phases (two grid barriers, index chasing through L2), not by "
                     "bandwidth: DESIGN.md section 5.",
@@ -597,6 +592,8 @@ def main():
     ap.add_argument("--solver", type=int, default=0, help="0 auto, 1 row-scan, 2 slot-stream")
     ap.add_argument("--sub", default="all", help="sub-records beside the headline: all | none | comma-separated workloads")
     ap.add_argument("--sub-steps", type=int, default=5)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the grants of the headline workload's last timed step to DIR/*.npy (float64)")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3

@@ -119,7 +119,7 @@ def run_sharded(args, rank, world, local):
             "cfg5_strong": big,
             "clocks": sampler.summary(),
             "parity": "tests/multi_gpu_check.py (every decision against one scheduler fed the whole queue; cfg5-1m against "
-                      "the reference's digest) -- profiles/r2_multi_gpu_parity.log",
+                      "the reference's digest)",
         }
         print(json.dumps(line))
     dist.barrier()

@@ -1,7 +1,7 @@
 /* minimal.c -- the ydsched C ABI from plain C: register two servants, decide a small queue,
  * renew and free the leases.  Links against any library that speaks the ABI:
  *
- *     gcc -std=c99 -Iinclude examples/minimal.c -o minimal -Lyadcc_b200 -lydsched      (B200)
+ *     gcc -std=c99 -Iinclude examples/minimal.c -o minimal -Lyadcc_b200 -lydsched      (H100)
  *
  * (the test-suite builds it against the CPU oracle to check that the headers are plain C and
  * that the calls behave as documented).  Mirrors what SchedulerServiceImpl does with

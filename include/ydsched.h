@@ -1,5 +1,5 @@
 /*
- * ydsched.h -- C ABI of the B200-native yadcc scheduler hot path.
+ * ydsched.h -- C ABI of the H100-native yadcc scheduler hot path.
  *
  * This is the drop-in boundary (SURVEY.md 8(b)): every entry point below
  * replaces one public method of the reference's `TaskDispatcher`
@@ -9,7 +9,7 @@
  * plain pointers, sizes and fixed-width integers only.
  *
  * Three shared libraries export exactly this ABI:
- *   - yadcc_b200/libydsched.so        host C++ + sm_100a CUDA kernels (the product)
+ *   - yadcc_b200/libydsched.so        host C++ + sm_90a CUDA kernels (the product)
  *   - oracle/libydoracle.so           CPU restatement of the algorithm (test infra)
  *   - oracle/_ref/libydref.so         the reference's own .cc files compiled
  *                                     verbatim against oracle/shim (test infra)
@@ -150,12 +150,12 @@ typedef struct yd_solve_stats {
 /* ---- lifecycle --------------------------------------------------------- */
 
 /* TaskDispatcher::TaskDispatcher (cc:78-88).  Returns NULL if the config is
- * malformed or (CUDA backend) no usable sm_100 device is present -- the CUDA
+ * malformed or (CUDA backend) no usable sm_90 device is present -- the CUDA
  * backend never falls back to a CPU path. */
 yd_sched* yd_create(const yd_config* cfg);
 /* TaskDispatcher::~TaskDispatcher (cc:90-92). */
 void yd_destroy(yd_sched* s);
-/* "cuda-sm100a", "oracle-port" or "reference". */
+/* "cuda-sm90a", "oracle-port" or "reference". */
 const char* yd_backend_name(void);
 /* yadcc::TryParseSize (yadcc/common/parse_size.cc:25-45).  Returns 1 and
  * stores the byte count on success, 0 when the reference returns nullopt. */

@@ -4,7 +4,7 @@
   ref   oracle/_ref/libydref.so    reference sources compiled verbatim (present
                                    when built in the dev container; travels to
                                    the GPU box as a prebuilt file)
-  cuda  yadcc_b200/libydsched.so   the product; needs a B200 -> @pytest.mark.gpu
+  cuda  yadcc_b200/libydsched.so   the product; needs an H100 -> @pytest.mark.gpu
 """
 import os
 import subprocess
@@ -22,7 +22,7 @@ CUDA_LIB = ROOT / "yadcc_b200" / "libydsched.so"
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run with -m gpu)")
 
 
 def _ensure_port():

@@ -4,15 +4,13 @@ import numpy as np
 import pytest
 
 from bloom_cases import run_bloom_suite, tu_keys
+from reference_results import check_reference
 
 
 @pytest.mark.parametrize("seed", range(3))
 def test_bloom_port_equals_reference(make_dispatcher, seed):
-    a = run_bloom_suite(make_dispatcher("ref"), seed)
-    b = run_bloom_suite(make_dispatcher("port"), seed)
-    assert len(a) == len(b)
-    for k, (x, y) in enumerate(zip(a, b)):
-        assert x.shape == y.shape and (x == y).all(), k
+    check_reference(f"bloom-{seed}", lambda: run_bloom_suite(make_dispatcher("ref"), seed),
+                    run_bloom_suite(make_dispatcher("port"), seed))
 
 
 @pytest.mark.parametrize("backend", ["port", "ref"])

@@ -363,7 +363,7 @@ def test_lease_ring_growth_and_window(make_dispatcher):
 
 def test_native_library_is_what_ran(make_dispatcher):
     d = make_dispatcher("cuda")
-    assert d.backend == "cuda-sm100a"
+    assert d.backend == "cuda-sm90a"
     w = S.config1()
     w.register(d)
     d.wait_for_starting_new_tasks(w.build_requests(d), 0.0)

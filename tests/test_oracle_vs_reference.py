@@ -1,6 +1,7 @@
 """The CPU restatement (oracle/port.cc) against the reference compiled verbatim
-(oracle/_ref) on seeded event streams, plus the committed golden digests that
-were generated from the verbatim build (tests/golden/make_golden.py)."""
+(oracle/_ref) on seeded event streams -- fingerprints of its results where it is not
+built (tests/reference_results.py) -- plus the committed golden digests that were
+generated from the verbatim build (tests/golden/make_golden.py)."""
 import json
 import os
 from pathlib import Path
@@ -8,28 +9,30 @@ from pathlib import Path
 import numpy as np
 import pytest
 
+from reference_results import check_reference
 from yadcc_b200 import streams as S
 
 GOLDEN = Path(__file__).parent / "golden"
 
 
+def _replay(make_dispatcher, kind, build):
+    d = make_dispatcher(kind)
+    return S.Replayer(d).run(build(d))
+
+
+def _port_equals_reference(make_dispatcher, key, build):
+    check_reference(key, lambda: _replay(make_dispatcher, "ref", build), _replay(make_dispatcher, "port", build))
+
+
 @pytest.mark.parametrize("seed", range(60))
 def test_fuzz_port_equals_reference(make_dispatcher, seed):
-    traces = []
-    for kind in ("ref", "port"):
-        d = make_dispatcher(kind)
-        st = S.fuzz_stream(d, seed, n_servants=8 + seed % 30, wide=(seed % 5 == 0))
-        traces.append(S.Replayer(d).run(st))
-    assert S.traces_equal(*traces), S.first_mismatch(*traces)
+    _port_equals_reference(make_dispatcher, f"fuzz-{seed}",
+                           lambda d: S.fuzz_stream(d, seed, n_servants=8 + seed % 30, wide=(seed % 5 == 0)))
 
 
 @pytest.mark.parametrize("name", ["cfg1", "cfg2-mod-small", "cfg2-random-small", "cfg3-small"])
 def test_configs_port_equals_reference(make_dispatcher, name):
-    traces = []
-    for kind in ("ref", "port"):
-        d = make_dispatcher(kind)
-        traces.append(S.Replayer(d).run(S.named_stream(name, d)))
-    assert S.traces_equal(*traces), S.first_mismatch(*traces)
+    _port_equals_reference(make_dispatcher, f"config-{name}", lambda d: S.named_stream(name, d))
 
 
 def test_port_matches_committed_golden_digests(make_dispatcher):
@@ -74,12 +77,13 @@ def test_dump_internals_port_equals_reference(make_dispatcher, seed):
     """TaskDispatcher::DumpInternals (task_dispatcher.cc:538-614): the per-servant rows and the five summary fields
     the reference's own function produces (written out by the harness from its Json::Value) against the
     restatement's -- after a stream that leaves servants in every state (full, low memory, not accepting, expired)."""
-    dumps = []
-    for kind in ("ref", "port"):
+    def dump(kind):
         d = make_dispatcher(kind)
         assert d.dump_internals() == {"servants_up": 0, "running_tasks": 0, "capacity": 0, "capacity_available": 0,
                                       "capacity_unavailable": 0}
         S.Replayer(d).run(S.fuzz_stream(d, seed, n_servants=10 + seed))
-        dumps.append(d.dump_internals())
-    assert dumps[0] == dumps[1]
-    assert len(dumps[0].get("servants", [])) == dumps[0]["servants_up"]
+        return d.dump_internals()
+
+    mine = dump("port")
+    check_reference(f"dump-internals-{seed}", lambda: dump("ref"), mine)
+    assert len(mine.get("servants", [])) == mine["servants_up"]

@@ -5,17 +5,15 @@ reference's literal loops over the verbatim TaskDispatcher (oracle/ref_harness.c
 import numpy as np
 import pytest
 
+from reference_results import check_reference
 from rpc_cases import run_rpc_stream
 from yadcc_b200 import Servant, _abi
 
 
 @pytest.mark.parametrize("seed", range(40))
 def test_rpc_expansion_port_equals_reference(make_dispatcher, seed):
-    a = run_rpc_stream(make_dispatcher("ref"), seed)
-    b = run_rpc_stream(make_dispatcher("port"), seed)
-    assert len(a) == len(b)
-    for x, y in zip(a, b):
-        assert x.shape == y.shape and (x == y).all()
+    check_reference(f"rpc-expansion-{seed}", lambda: run_rpc_stream(make_dispatcher("ref"), seed),
+                    run_rpc_stream(make_dispatcher("port"), seed))
 
 
 @pytest.mark.parametrize("backend", ["port", "ref"])

@@ -2,16 +2,14 @@
 loops run literally over the verbatim TaskDispatcher/RunningTaskBookkeeper (oracle/_ref)."""
 import pytest
 
+from reference_results import check_reference
 from running_index_cases import reference_test_case, run_suite
 
 
 @pytest.mark.parametrize("seed", range(4))
 def test_running_index_port_equals_reference(make_dispatcher, seed):
-    a = run_suite(make_dispatcher("ref"), seed)
-    b = run_suite(make_dispatcher("port"), seed)
-    assert len(a) == len(b)
-    for k, (x, y) in enumerate(zip(a, b)):
-        assert x.shape == y.shape and (x == y).all(), k
+    check_reference(f"running-index-{seed}", lambda: run_suite(make_dispatcher("ref"), seed),
+                    run_suite(make_dispatcher("port"), seed))
 
 
 @pytest.mark.parametrize("backend", ["port", "ref"])

@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 import service_cases as SC
+from reference_results import check_reference
 
 CASES = [SC.token_case, SC.token_with_intersection_case, SC.token_without_intersection_case, SC.heartbeat_rules_case,
          SC.lease_flow_case, SC.token_rollout_case]
@@ -22,9 +23,7 @@ def _same(a, b):
 
 @pytest.mark.parametrize("case", CASES, ids=lambda c: c.__name__)
 def test_service_case(make_dispatcher, case):
-    a = case(make_dispatcher("ref"))
-    b = case(make_dispatcher("port"))
-    assert _same(a, b)
+    check_reference(f"service-{case.__name__}", lambda: case(make_dispatcher("ref")), case(make_dispatcher("port")))
 
 
 def test_service_needs_both_token_lists(make_dispatcher):

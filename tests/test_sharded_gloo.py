@@ -170,7 +170,7 @@ def test_range_sharded_queue_on_two_gloo_ranks_equals_one_scheduler(tmp_path, po
     """The range-sharded scheduler's contract (include/ydshard.h) on CPU: two gloo ranks, each with its contiguous
     range of one FIFO queue and a replica of the servant table, make together exactly the decisions -- statuses,
     servants, FIFO task ids, per-servant bookkeeping -- of one TaskDispatcher fed the whole queue, across a
-    collective FreeTask.  (On B200s the exchange is the C++/NCCL path; tests/multi_gpu_check.py checks that one.)"""
+    collective FreeTask.  (On GPUs the exchange is the C++/NCCL path; tests/multi_gpu_check.py checks that one.)"""
     import torch.multiprocessing as mp
     from yadcc_b200 import TaskDispatcher
     from yadcc_b200 import streams as S

@@ -5,13 +5,12 @@ import pytest
 
 pytest.importorskip("google.protobuf")
 
+from reference_results import check_reference
 from wire_cases import run_wire_scenario
 
 
 def test_wire_scenario_port_equals_reference(make_dispatcher):
-    a = run_wire_scenario(make_dispatcher, "ref")
-    b = run_wire_scenario(make_dispatcher, "port")
-    assert a == b
+    check_reference("wire-scenario", lambda: run_wire_scenario(make_dispatcher, "ref"), run_wire_scenario(make_dispatcher, "port"))
 
 
 def test_wire_parser_survives_mutated_frames(make_dispatcher):
@@ -90,8 +89,8 @@ def test_wire_request_counts_are_not_trusted(make_dispatcher):
     from yadcc_b200.service import SchedulerService
 
     PB = W.PB
-    results = []
-    for kind in ("port", "ref"):
+
+    def scenario(kind):
         d = make_dispatcher(kind)
         svc = SchedulerService(d, acceptable_user_tokens="usr", acceptable_servant_tokens="srv", token_seed=2)
         dg = "d" * 64
@@ -109,11 +108,13 @@ def test_wire_request_counts_are_not_trusted(make_dispatcher):
         resp = PB["WaitForStartingTaskResponse"]()
         resp.ParseFromString(body)
         assert st == 0 and len(resp.grants) == 20  # 5 servants x max_tasks 4
-        results.append([(g.task_grant_id, g.servant_location) for g in resp.grants])
+        grants = [(g.task_grant_id, g.servant_location) for g in resp.grants]
         # and the same two as frames in one batch
         frames = [(W.request_frame("WaitForStartingTask", bad, 7), "172.16.0.1"),
                   (W.request_frame("WaitForStartingTask", good, 8), "172.16.0.1")]
         out = svc.handle_frames(frames, now=1.5)
         assert [o[2] for o in out] == [1003, 1001]  # the pool is full now: NO_QUOTA for the good caller
         svc.close()
-    assert results[0] == results[1]
+        return grants
+
+    check_reference("wire-request-counts", lambda: scenario("ref"), scenario("port"))

@@ -69,7 +69,7 @@ def main():
             "warm_bytes": sum(k["dram_read"] + k["dram_write"] for k in warm),
             "sum_kernel_us": round(sum(k["us"] for k in warm), 1),
             "sum_kernel_us_cold": round(sum(k["us"] for k in cold), 1),
-            "source": "profiles/r2f_dram_traffic.json (tools/ncu_traffic.py on a B200)",
+            "source": "tools/ncu_traffic.py",
             "launches_warm": warm, "launches_cold": cold,
         }
         with open(OUT / f"r2f_launches_{w}.csv", "w") as f:

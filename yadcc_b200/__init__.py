@@ -1,8 +1,8 @@
-"""yadcc_b200 -- B200-native implementation of yadcc's scheduler hot path.
+"""yadcc_b200 -- H100-native implementation of yadcc's scheduler hot path.
 
 Only what the path needs lives here:
 
-  csrc/            host C++ + sm_100a CUDA kernels behind include/ydsched.h
+  csrc/            host C++ + sm_90a CUDA kernels behind include/ydsched.h
   _abi.py          ctypes declarations of that C ABI
   dispatcher.py    host-side mirror of the reference's `TaskDispatcher`
                    interface (yadcc/scheduler/task_dispatcher.h:120-181)

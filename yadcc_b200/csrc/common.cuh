@@ -1,4 +1,4 @@
-// common.cuh -- shared definitions for the sm_100a scheduler kernels.
+// common.cuh -- shared definitions for the sm_90a scheduler kernels.
 //
 // HBM layout (all arrays are structure-of-arrays, indexed by REGISTRY POSITION,
 // i.e. the reference's `servants_.servants` vector index, whose order is the

@@ -2,7 +2,7 @@
 //
 // At the headline size (100 k requests x 2 k servants) every kernel of the pipeline in ydsched.cu:LaunchStream does a
 // few microseconds of work and costs a few more to launch and drain: ten dependent kernels are ten launch latencies
-// (profiles/r2_launches_cfg2-mod.csv: 13 kernels, sum 88 us, ~3.6 us for a kernel that does nothing).  Here the same
+// (the kernel-by-kernel pipeline is 13 kernels per solve).  Here the same
 // device functions (classes.cuh, parallel.cuh, tasks.cuh) run as phases of one co-resident grid -- one block of 1024
 // threads per SM, tiles handed out round-robin -- separated by grid barriers:
 //

@@ -1,4 +1,4 @@
-// ydsched.cu -- host side of the B200-native scheduler hot path and its C ABI
+// ydsched.cu -- host side of the H100-native scheduler hot path and its C ABI
 // (include/ydsched.h).  This translation unit owns:
 //
 //   * the servant registry mirror (strings, digests, leases) -- the part of
@@ -11,7 +11,7 @@
 //     tasks.cuh.  All arithmetic of the hot path (eligibility, capacity,
 //     utilisation, pick, task ids, leases, sweeps) runs on the GPU.
 //
-// There is no CPU fallback: yd_create fails without an sm_100 device.
+// There is no CPU fallback: yd_create fails without an sm_90 device.
 #include <algorithm>
 #include <chrono>
 #include <cstdio>
@@ -544,7 +544,7 @@ void yd_sched::FetchCounters() {
 
 extern "C" {
 
-const char* yd_backend_name(void) { return "cuda-sm100a"; }
+const char* yd_backend_name(void) { return "cuda-sm90a"; }
 
 int yd_parse_size(const char* text, uint64_t* out_bytes) { return ParseSize(text, out_bytes) ? 1 : 0; }
 
@@ -561,8 +561,8 @@ yd_sched* yd_create(const yd_config* cfg) {
   }
   cudaDeviceProp prop{};
   YD_CUDA_CHECK(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major < 10) {
-    fprintf(stderr, "ydsched: device %d is sm_%d%d; kernels are built for sm_100a only\n", cfg->device,
+  if (prop.major != 9 || prop.minor != 0) {  // sm_90a code loads on compute capability 9.0 and nothing else
+    fprintf(stderr, "ydsched: device %d is sm_%d%d; kernels are built for sm_90a only\n", cfg->device,
             prop.major, prop.minor);
     return nullptr;
   }
@@ -597,7 +597,7 @@ yd_sched* yd_create(const yd_config* cfg) {
     YD_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, cfg->device));
     YD_CUDA_CHECK(cudaFuncSetAttribute(yd::k_fused_front, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
     YD_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, yd::k_fused_front, 1024, 64 * 1024));
-    s->fused_grid = per_sm >= 1 ? (uint32_t)sms : 0u;  // (0: the kernel does not fit an SM -- never on sm_100a; the pipeline is used)
+    s->fused_grid = per_sm >= 1 ? (uint32_t)sms : 0u;  // (0: the kernel does not fit an SM -- never on sm_90a; the pipeline is used)
   }
   s->dump_env = getenv("YDSCHED_DUMP") != nullptr;
   s->debug_env = getenv("YDSCHED_DEBUG") != nullptr;
@@ -1417,8 +1417,8 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
   const uint32_t Nb = (uint32_t)NextPow2(N, 1024);
   // The slot table: kept across solves (all running_tasks values of every servant) while it is small enough,
   // else rebuilt per solve and clamped to the batch size.
-  // Merge-solver chunk: more, shorter chunks pay while the request-side passes are short (measured on a B200: cfg2-random
-  // 306 vs 349 us, cfg-self 181 vs 199 us at 256 vs 512 slots; at 1 M requests 551 vs 515 us)
+  // Merge-solver chunk: more, shorter chunks pay while the request-side passes are short (measured on an H100 SXM, 700 W:
+  // cfg2-random 324 vs 374 us, cfg-self 177 vs 187 us at 256 vs 512 slots; cfg3, 1 M requests, 604 vs 573 us)
   if (s->merge_chunk_auto && !s->shard) s->merge_chunk = Nb <= 262144 ? 256u : 512u;
   const size_t static_bound = S ? s->static_bound_cache : 0;  // (= StaticSlotBound(s), kept by SyncFacts)
   const bool want_static = s->solver_pref != 1 && static_bound <= kStaticSlotLimit;

@@ -141,7 +141,7 @@ class TaskDispatcher:
         if not self._h:
             raise RuntimeError(
                 f"yd_create failed for backend {self.backend!r} ({self._lib._yd_path}); "
-                "the CUDA backend needs an sm_100 GPU and never falls back to the CPU"
+                "the CUDA backend needs an sm_90 GPU (H100) and never falls back to the CPU"
             )
         self._env_ids: dict[str, int] = {}
         self._ip_ids: dict[str, int] = {}

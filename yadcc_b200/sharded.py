@@ -24,7 +24,7 @@ the caller-visible `owner_of_*` maps.
 
 The class is backend-agnostic (any library speaking the ydsched C ABI) and
 transport-agnostic (any torch.distributed backend), so the N>1 logic is tested on CPU
-with gloo + the oracle and runs unchanged with NCCL on B200s.
+with gloo + the oracle and runs unchanged with NCCL on H100s.
 """
 from __future__ import annotations
 

@@ -134,6 +134,26 @@ __device__ __forceinline__ void cls_insert_one(uint32_t env, uint32_t mv, uint32
   }
 }
 
+// A request's class in the table a previous solo solve kept (fused.cuh, speculative variant), or kNone for an unknown
+// digest or one no component holds (EnvironmentNotFound, as cls_insert_one skips them).  `miss`: the kept table cannot
+// decide the request -- its class is not in the table, or the requestor's IP is that of a servant of the component
+// (which would take it off the data-parallel path).
+__device__ __forceinline__ uint32_t kept_class(uint32_t env, uint32_t mv, uint32_t ip, const TopoView& t,
+                                               const ClassTable& ct, bool& miss) {
+  if (env >= t.n_envs) return kNone;
+  const uint32_t comp = t.env_comp[env];
+  if (comp == kNone) return kNone;
+  const uint32_t slot = cls_find(ct.keys, ((unsigned long long)env << 32) | mv);
+  const uint32_t cls = slot != kNone ? ct.slot_cls[slot] : kNone;
+  if (cls == kNone) miss = true;
+  if (ip < t.n_ips) {
+    for (uint32_t u = t.ip_off[ip], e = t.ip_off[ip + 1]; u < e; ++u) {
+      if (t.sv_comp[t.ip_sv[u]] == comp) miss = true;
+    }
+  }
+  return cls;
+}
+
 __global__ void __launch_bounds__(256) k_cls_insert(const yd_task_req* __restrict__ reqs,
                                                     const DynParams* __restrict__ dp, TopoView t, ClassTable ct) {
   __shared__ unsigned long long s_seen[64];

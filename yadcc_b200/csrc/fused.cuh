@@ -13,12 +13,31 @@
 //   P5  per-class sorted slot lists                                 (list_fill_tile)
 //   B3  barrier
 //   P6  verdicts of the data-parallel components, FIFO records of the merge components (rank_assign_one) and --
-//       `solo`, when every component with requests is data-parallel -- task ids (look-back scan over the tiles),
-//       grants, leases, ++running_tasks (final_tile): the whole solve in one launch.
+//       `solo`, when every component with requests is data-parallel -- task ids (in closed form from the per-class
+//       counts, see fused_class_grants), grants, leases, ++running_tasks (final_tile): the whole solve in one launch.
 //
 // Not solo: res[] goes to HBM and the merge / sequential solvers and k_final_fused follow as separate launches.
 // A solo kernel that finds a component it cannot decide raises flag 4 and decides nothing; the host replays the batch
 // with the general sequence (and remembers which one the workload needs).
+//
+// E1 only numbers the classes, and a scheduler's class set -- (digest, min_version) pairs -- rarely changes from one
+// batch to the next.  So a solo solve whose class set is the one of the previous solo solve KEEPS its class table (keys,
+// slot_cls, cls_env / mv / comp, meta, comp_mode), and the next solo solve runs SPECULATIVELY on it, with one barrier:
+//
+//   A   every request looked up in the kept table (kept_class) and ranked in its tile (rank_in_tile): its class and rank
+//       stay in registers, as tile t is handled by block t % G in both phases; list ballots and counts; eligible
+//       servants per class (servant versions and max_tasks change without a new topology)
+//   --  barrier
+//   B   P6 as above (the lite selection, closed-form task ids).  The last block resets the barrier words, nothing else.
+//
+// A request MISSES when its digest is held by a component but its class is not in the table, or when its IP is that of
+// a servant of its component: flag kFlagSpecMiss, nothing is decided, the last block clears the scratch (the kept table
+// too) and the host replays the batch without speculation.  Why a hit decides exactly what a full solve decides: a kept
+// table was written by a completed solo solve, so each of its components holds one class and is data-parallel.  If
+// every request hits and none comes from a servant of its component, each component with requests still has exactly
+// that one class and no self-request, and cls_finalize_block would pick the same modes; a kept class without requests
+// only makes a component without requests, which decides nothing (and grants nothing: min(0, L) = 0).  Class ids do not
+// enter decisions: ranks and lists are per class.
 //
 // The barrier is the cooperative-groups pattern (bar.sync; one thread: fence, atomic arrive, spin, fence; bar.sync).  The
 // grid never exceeds the number of SMs, so all blocks are resident; a block that has to wait for other kernels to drain
@@ -41,6 +60,9 @@ struct FusedScalars {
   // (written by the last phase of a solo solve) -- no copy-engine transfer before or after the kernel.  Else null.
   const void* zc_in;
   void* zc_out;
+  // Solo, not speculative: the class-set fingerprint of the previous such solve (0: none).  A solve that finds the same
+  // class set again keeps its class table for the speculative variant; any other leaves the scratch clean.
+  unsigned long long kept_fp;
 };
 
 // The solo kernel's result, in MAPPED pinned host memory (posted writes; the host reads it after the stream has drained):
@@ -49,7 +71,17 @@ struct FusedHostIO {
   unsigned long long done_seq;   // = the launch's seq once the record below is complete (written last)
   unsigned long long granted;    // grants of the batch
   uint32_t meta[8];              // the class table's meta words (meta[1] != 0: nothing was decided, see ClassTable)
+  unsigned long long classes_fp; // solo, not speculative: fingerprint of the batch's class set (fused_classes_fp)
 };
+
+// Flag (meta[1]) of a speculative solve that met a request the kept class table cannot decide: nothing was decided, the
+// scratch is clean, the host replays the batch without speculation.
+constexpr uint32_t kFlagSpecMiss = 5;
+
+// What a completed solo solve keeps of its class table for the next, speculative one: the keys (behind res[]), comp_mode,
+// and the head of the class region (MakeClassTable's layout): slot_cls, meta, cls_env, cls_mv, cls_comp.
+constexpr uint32_t kKeptClsWords = kClsTableSize + 8 + 3 * kMaxClasses;
+static_assert(kKeptClsWords % 4 == 0, "the scratch behind the kept words is cleared in 16-byte words");
 
 struct FusedArgs {
   FusedScalars sc;              // by value ...
@@ -85,7 +117,6 @@ struct FusedArgs {
   uint32_t* bar;  // [3], zeroed per solve: arrivals, release epoch, blocks that are done
   // solo
   uint32_t solo, packed_out;
-  unsigned long long* look;
   const uint32_t* comp_sv;
   TaskRing ring;
   void* out;
@@ -93,6 +124,7 @@ struct FusedArgs {
   uint32_t n_servants;
   uint32_t loff_cache_words;  // dynamic shared memory of the launch, in words
   uint32_t lite;              // solo: no leader scans -- every block derives the offsets it needs from the raw counts
+  uint32_t spec;              // solo, speculative: the class table kept from the last solo solve, one grid barrier
   unsigned long long* prof;  // debug (YDSCHED_FUSED_PROF): block 0 stamps %globaltimer at every phase boundary, else null
 };
 
@@ -169,14 +201,45 @@ __device__ __forceinline__ bool fused_done_last(uint32_t* bar) {
   return s_fin != 0;
 }
 
+// Sum of `v` over the block (1024 threads), returned to every thread.
+__device__ __forceinline__ uint32_t fused_block_sum(uint32_t v) {
+  __shared__ uint32_t s_part[32];
+  const uint32_t lane = threadIdx.x & 31;
+  v = __reduce_add_sync(0xffffffffu, v);
+  __syncthreads();  // (s_part of the previous call has been read)
+  if (lane == 0) s_part[threadIdx.x >> 5] = v;
+  __syncthreads();
+  return __reduce_add_sync(0xffffffffu, s_part[lane]);
+}
+
 // The result record for the host (threads 0..8 of one block): the class table's meta words and the grant count, as
 // posted writes into mapped host memory -- or, `report_dev`, into HBM for a copy node to fetch.  The host reads it after
 // the stream has drained, so no ordering is needed among the writes.
-__device__ __forceinline__ void fused_report(const FusedArgs& a, unsigned long long seq, unsigned long long granted) {
+__device__ __forceinline__ void fused_report(const FusedArgs& a, unsigned long long seq, unsigned long long granted,
+                                             unsigned long long fp = 0) {
   FusedHostIO* h = a.hio;
   const uint32_t k = threadIdx.x;
   if (k < 8) h->meta[k] = a.ct.meta[k];
-  else if (k == 8) { h->granted = granted; h->done_seq = seq; }
+  else if (k == 8) { h->granted = granted; h->classes_fp = fp; h->done_seq = seq; }
+}
+
+// Order-independent fingerprint of the class set (the occupied keys of the class table), by one block of 1024 threads:
+// the number of classes in the high word, a sum of mixed keys in the low word -- never 0.
+__device__ __forceinline__ unsigned long long fused_classes_fp(const unsigned long long* __restrict__ keys) {
+  uint32_t cnt = 0, mix = 0;
+  for (uint32_t i = threadIdx.x; i < kClsTableSize; i += 1024) {
+    const unsigned long long k = keys[i];
+    if (k != kClsEmpty) {
+      unsigned long long x = k * 0x9e3779b97f4a7c15ull;
+      x ^= x >> 31;
+      x *= 0xbf58476d1ce4e5b9ull;
+      mix += (uint32_t)(x >> 32);
+      ++cnt;
+    }
+  }
+  cnt = fused_block_sum(cnt);
+  mix = fused_block_sum(mix);
+  return ((unsigned long long)(cnt + 1) << 32) | mix;
 }
 
 // In-place exclusive scan of data[0 .. cells) by one block of 1024 threads (8 values per thread and round).
@@ -266,13 +329,12 @@ __device__ __forceinline__ uint32_t fused_select(uint32_t q, const FusedArgs& a,
 
 // The same with block-local tables built from the RAW counts (no scan by a leader): `rows` = per class the exclusive
 // offsets of its slot tiles + its total (n_ltiles + 1 words per class), `rpre[c]` = class-c requests in the request tiles
-// before this one.
-__device__ __forceinline__ uint32_t fused_select_lite(uint32_t q, const FusedArgs& a, const uint32_t* __restrict__ rows,
-                                                       const uint32_t* __restrict__ rpre) {
-  const uint32_t c = a.rcls[q];
+// before this one; c / rank = the request's class and its rank among the class's requests of its tile.
+__device__ __forceinline__ uint32_t fused_select_lite(uint32_t c, uint32_t rank, const FusedArgs& a,
+                                                       const uint32_t* __restrict__ rows, const uint32_t* __restrict__ rpre) {
   if (c == kNone) return kResEnvNotFound;
   if (a.ct.cls_nelig[c] == 0) return kResEnvNotFound;  // cc:105-108
-  const uint32_t target = rpre[c] + a.rrank[q];
+  const uint32_t target = rpre[c] + rank;
   const uint32_t* row = rows + c * (a.n_ltiles + 1);
   if (target >= row[a.n_ltiles]) return kResTimeout;   // cc:116-118
   uint32_t lo = 0, hi = a.n_ltiles;
@@ -301,16 +363,65 @@ __device__ __forceinline__ uint32_t fused_select_lite(uint32_t q, const FusedArg
   return a.dec.rec[lo * kListTile + w * 32 + bit].x;
 }
 
+// Task ids of a solo solve in closed form.  The selections above grant the class-c request with class rank k exactly
+// when cls_nelig[c] != 0 && k < L_c (L_c = the length of c's list), so of the `before` class-c requests in the tiles
+// before a tile, min(before, L_c) were granted; summed over the classes that is the tile's first FIFO ordinal.  Every
+// block derives it from the count matrices it already holds: no tile waits for another.
+__device__ __forceinline__ uint32_t fused_class_grants(const FusedArgs& a, uint32_t c, uint32_t before, uint32_t len) {
+  return a.ct.cls_nelig[c] != 0 ? min(before, len) : 0u;
+}
+
+// Request q = tile * 1024 + thread (a block of 1024 threads): its digest id, min_version and requestor IP; false beyond
+// the queue's end.  A zero-copy solve first copies the tile from the caller's page-locked array to HBM (every later read
+// of the requests, here and in the kernels that follow, hits the copy); a packed upload is also written out as the
+// 24-byte records the kernels after this one read (not solo).
+__device__ __forceinline__ bool fused_fetch_req(const FusedArgs& a, const ReqView& rv, const char* zc_in, uint32_t tile,
+                                                uint32_t n, uint32_t& env, uint32_t& mv, uint32_t& ip) {
+  const uint32_t tid = threadIdx.x, q = tile * 1024 + tid;
+  if (zc_in) {
+    // 16 bytes per thread and step (coalesced reads over PCIe)
+    if (a.reqs16) {
+      if (q < n) a.reqs16_w[q] = reinterpret_cast<const uint4*>(zc_in)[q];
+    } else {
+      const uint32_t bytes = min(n - tile * 1024, 1024u) * (uint32_t)sizeof(yd_task_req);  // a multiple of 8
+      const char* src = zc_in + size_t(tile) * 1024 * sizeof(yd_task_req);
+      char* dst = reinterpret_cast<char*>(const_cast<yd_task_req*>(a.reqs)) + size_t(tile) * 1024 * sizeof(yd_task_req);
+      for (uint32_t o = tid * 16; o < bytes; o += 1024 * 16) {
+        if (o + 16 <= bytes) *reinterpret_cast<uint4*>(dst + o) = *reinterpret_cast<const uint4*>(src + o);
+        else *reinterpret_cast<uint2*>(dst + o) = *reinterpret_cast<const uint2*>(src + o);
+      }
+    }
+    __syncthreads();
+  }
+  if (q >= n) return false;
+  if (a.reqs16) {
+    const uint4 w = a.reqs16[q];
+    env = w.x; mv = w.y; ip = w.z;
+    if (a.reqs_w) {
+      uint2* dst = reinterpret_cast<uint2*>(a.reqs_w + q);
+      const unsigned long long ns = (unsigned long long)(w.w & 0x7fffffffu) * 1000000ull;
+      dst[0] = make_uint2(env, mv);
+      dst[1] = make_uint2(ip, (w.w >> 31) ? YD_REQ_FLAG_PREFETCH : 0u);
+      dst[2] = make_uint2((uint32_t)ns, (uint32_t)(ns >> 32));
+    }
+  } else {
+    rv.head(q, env, mv);
+    ip = rv.ip(q);
+  }
+  return true;
+}
+
 __global__ void __launch_bounds__(1024, 1) k_fused_front(FusedArgs a) {
   extern __shared__ uint32_t s_loff[];  // solo: the scanned list offsets, when a.loff_cache_words holds them
   __shared__ unsigned long long s_seen[64];
   __shared__ DynParams s_dyn;
-  __shared__ unsigned long long s_seq, s_zc_in, s_zc_out;
+  __shared__ unsigned long long s_seq, s_zc_in, s_zc_out, s_kept_fp;
   const uint32_t tid = threadIdx.x, G = gridDim.x;
   if (tid == 0) {
     const FusedScalars sc = a.sc_dev ? *a.sc_dev : a.sc;
     s_dyn = sc.dyn;
     s_seq = sc.seq;
+    s_kept_fp = sc.kept_fp;
     s_zc_in = reinterpret_cast<unsigned long long>(sc.zc_in);
     s_zc_out = reinterpret_cast<unsigned long long>(sc.zc_out);
     if (blockIdx.x == 0 && a.dyn_out) *a.dyn_out = sc.dyn;
@@ -323,11 +434,11 @@ __global__ void __launch_bounds__(1024, 1) k_fused_front(FusedArgs a) {
   const ReqView rv{a.reqs, a.reqs16};
 
   fused_stamp(a, 0);
-  // ---- P1: classes ---------------------------------------------------------------------------------------------
   if (tid < 64) s_seen[tid] = kClsEmpty;
   __syncthreads();
   {
     const size_t S4 = size_t(a.n_servants) * 4;
+    if (a.spec) fused_prefetch(a.ct.keys, kClsTableSize * 8);
     fused_prefetch(a.dec.rec, size_t(m) * 8);
     fused_prefetch(a.sv.run, S4);
     fused_prefetch(a.sv.version, S4);
@@ -339,42 +450,56 @@ __global__ void __launch_bounds__(1024, 1) k_fused_front(FusedArgs a) {
     else { fused_prefetch(a.t.sv_env_off, S4 + 4); }
   }
   const char* zc_in = reinterpret_cast<const char*>(s_zc_in);
+  uint32_t ncls, nlists;
+  bool lite;
+  // speculative: class | in-tile rank << 16 of this thread's request in the block's first / second request tile
+  uint32_t spec_cr0 = 0xffffu, spec_cr1 = 0xffffu;
+  if (a.spec) {
+    // ---- A: requests against the kept class table, list ballots and counts, eligible servants per class ------------
+    // Request tiles are the first items, so tile t is handled by block t % G here and in B below: the class and rank of
+    // a request stay in this thread's registers.
+    ncls = min(a.ct.meta[0], a.ct.cls_bound);
+    nlists = min(a.ct.meta[3], a.ct.cls_bound);
+    bool miss = false;
+    const uint32_t items = nb_live + lt_live + ncls;
+    for (uint32_t it = blockIdx.x, k = 0; it < items; it += G, ++k) {
+      if (it < nb_live) {
+        uint32_t env, mv, ip, cls = kNone;
+        if (fused_fetch_req(a, rv, zc_in, it, n, env, mv, ip)) cls = kept_class(env, mv, ip, a.t, a.ct, miss);
+        const uint32_t rank = rank_in_tile(it, cls, a.ct, a.n_rtiles, a.rank_cnt);
+        const uint32_t cr = (rank << 16) | (cls & 0xffffu);
+        if (k == 0) spec_cr0 = cr;
+        else if (k == 1) spec_cr1 = cr;
+        else miss = true;  // (more request tiles than two per block: the host does not speculate on such batches)
+      } else if (it < nb_live + lt_live) {
+        list_count_tile(it - nb_live, m, a.dec, a.t, a.ct, a.sv, a.n_ltiles, a.list_cnt, a.list_bal);
+      } else {
+        cls_elig_class(it - nb_live - lt_live, a.t, a.ct, a.sv);
+      }
+    }
+    // slot tiles beyond the table's end hold no members (the lists' row scans below read them; nothing re-zeroes them)
+    const uint32_t tail = a.n_ltiles - lt_live;
+    for (uint32_t i = blockIdx.x * 1024 + tid; i < nlists * tail; i += G * 1024) a.list_cnt[(i / tail) * a.n_ltiles + lt_live + i % tail] = 0;
+    if (__syncthreads_or(miss) && tid == 0) atomicExch(&a.ct.meta[1], kFlagSpecMiss);
+    lite = true;  // (the host speculates only when the lists' offsets fit in shared memory)
+    fused_stamp(a, 1);
+    fused_barrier(a.bar, 1);
+    fused_stamp(a, 2);
+    if (*reinterpret_cast<volatile uint32_t*>(&a.ct.meta[1]) != 0) {
+      // nothing is decided: the last block reports and leaves the scratch clean (the kept table too) for the replay
+      if (fused_done_last(a.bar)) {
+        fused_report(a, s_seq, 0);
+        __syncthreads();  // (the report reads meta[], which lies in the region zeroed below)
+        for (uint32_t i = tid; i < kClsTableSize; i += 1024) a.clean_keys[i] = kClsEmpty;
+        for (uint32_t i = tid; i < a.clean_zero_vec; i += 1024) a.clean_zero[i] = make_uint4(0u, 0u, 0u, 0u);
+      }
+      return;
+    }
+  } else {
+  // ---- P1: classes ---------------------------------------------------------------------------------------------
   for (uint32_t tile = blockIdx.x; tile < nb_live; tile += G) {
-    const uint32_t q = tile * 1024 + tid;
-    if (zc_in) {
-      // this tile of the caller's page-locked array -> HBM, 16 bytes per thread and step (coalesced reads over PCIe);
-      // every later read of the requests, here and in the kernels that follow, hits the copy
-      if (a.reqs16) {
-        if (q < n) a.reqs16_w[q] = reinterpret_cast<const uint4*>(zc_in)[q];
-      } else {
-        const uint32_t bytes = min(n - tile * 1024, 1024u) * (uint32_t)sizeof(yd_task_req);  // a multiple of 8
-        const char* src = zc_in + size_t(tile) * 1024 * sizeof(yd_task_req);
-        char* dst = reinterpret_cast<char*>(const_cast<yd_task_req*>(a.reqs)) + size_t(tile) * 1024 * sizeof(yd_task_req);
-        for (uint32_t o = tid * 16; o < bytes; o += 1024 * 16) {
-          if (o + 16 <= bytes) *reinterpret_cast<uint4*>(dst + o) = *reinterpret_cast<const uint4*>(src + o);
-          else *reinterpret_cast<uint2*>(dst + o) = *reinterpret_cast<const uint2*>(src + o);
-        }
-      }
-      __syncthreads();
-    }
-    if (q < n) {
-      uint32_t env, mv, ip;
-      if (a.reqs16) {
-        const uint4 w = a.reqs16[q];
-        env = w.x; mv = w.y; ip = w.z;
-        if (a.reqs_w) {  // the kernels after this one read 24-byte records
-          uint2* dst = reinterpret_cast<uint2*>(a.reqs_w + q);
-          const unsigned long long ns = (unsigned long long)(w.w & 0x7fffffffu) * 1000000ull;
-          dst[0] = make_uint2(env, mv);
-          dst[1] = make_uint2(ip, (w.w >> 31) ? YD_REQ_FLAG_PREFETCH : 0u);
-          dst[2] = make_uint2((uint32_t)ns, (uint32_t)(ns >> 32));
-        }
-      } else {
-        rv.head(q, env, mv);
-        ip = rv.ip(q);
-      }
-      cls_insert_one(env, mv, ip, a.t, a.ct, s_seen);
-    }
+    uint32_t env, mv, ip;
+    if (fused_fetch_req(a, rv, zc_in, tile, n, env, mv, ip)) cls_insert_one(env, mv, ip, a.t, a.ct, s_seen);
   }
 
   fused_stamp(a, 1);
@@ -392,8 +517,8 @@ __global__ void __launch_bounds__(1024, 1) k_fused_front(FusedArgs a) {
     if (a.solo && blockIdx.x == 0) fused_report(a, s_seq, 0);
     return;
   }
-  const uint32_t ncls = min(a.ct.meta[0], a.ct.cls_bound);
-  const uint32_t nlists = min(a.ct.meta[3], a.ct.cls_bound);
+  ncls = min(a.ct.meta[0], a.ct.cls_bound);
+  nlists = min(a.ct.meta[3], a.ct.cls_bound);
   fused_stamp(a, 2);
 
   // ---- P3: rank counts, list ballots and counts, eligible servants per class ---------------------------------------
@@ -417,7 +542,7 @@ __global__ void __launch_bounds__(1024, 1) k_fused_front(FusedArgs a) {
 
   fused_stamp(a, 3);
   // ---- E2: both count matrices -> offsets (class-major, tile-minor, + the end cell) -------------------------------
-  const bool lite = a.solo && a.lite && nlists * (a.n_ltiles + 1) <= a.loff_cache_words;  // (the same in every block)
+  lite = a.solo && a.lite && nlists * (a.n_ltiles + 1) <= a.loff_cache_words;  // (the same in every block)
   if (lite) {
     fused_barrier(a.bar, 2);  // the counts stay raw: each block derives what it needs below
   } else if (fused_arrive(a.bar, 2)) {
@@ -426,6 +551,7 @@ __global__ void __launch_bounds__(1024, 1) k_fused_front(FusedArgs a) {
     fused_release(a.bar, 2);
   } else {
     fused_wait(a.bar, 2);
+  }
   }
 
   fused_stamp(a, 4);
@@ -469,19 +595,29 @@ __global__ void __launch_bounds__(1024, 1) k_fused_front(FusedArgs a) {
       }
       if (lane == 0) s_loff[c * stride + a.n_ltiles] = running;
     }
-    for (uint32_t tile = blockIdx.x; tile < nb_live; tile += G) {
+    for (uint32_t tile = blockIdx.x, k = 0; tile < nb_live; tile += G, ++k) {
       __syncthreads();  // (s_loff is complete; s_rpre of the previous tile has been consumed)
+      uint32_t before = 0;  // (lane 0 of each warp) grants of its classes in the tiles before this one
       for (uint32_t c = warp; c < ncls; c += 32) {  // class-c requests in the tiles before this one
         uint32_t sum = 0;
         for (uint32_t t = lane; t < tile; t += 32) sum += a.rank_cnt[c * a.n_rtiles + t];
         sum = __reduce_add_sync(0xffffffffu, sum);
-        if (lane == 0) s_rpre[c] = sum;
+        if (lane == 0) {
+          s_rpre[c] = sum;
+          before += fused_class_grants(a, c, sum, s_loff[c * stride + a.n_ltiles]);
+        }
       }
-      __syncthreads();
+      const uint32_t base = fused_block_sum(before);  // (also the barrier that publishes s_rpre)
       const uint32_t q = tile * 1024 + tid;
-      const uint32_t r = q < n ? fused_select_lite(q, a, s_loff, s_rpre) : kResEnvNotFound;
-      if (a.packed_out) final_tile<true, true, true>(tile, nb_live - 1, r, n, now_ns, rv, a.look, a.comp_sv, ring, out, a.counters, a.sv.run, a.sv.ever);
-      else final_tile<false, true, true>(tile, nb_live - 1, r, n, now_ns, rv, a.look, a.comp_sv, ring, out, a.counters, a.sv.run, a.sv.ever);
+      uint32_t r = kResEnvNotFound;
+      if (q < n && a.spec) {
+        const uint32_t cr = k == 0 ? spec_cr0 : spec_cr1, c = cr & 0xffffu;
+        r = fused_select_lite(c == 0xffffu ? kNone : c, cr >> 16, a, s_loff, s_rpre);
+      } else if (q < n) {
+        r = fused_select_lite(a.rcls[q], a.rrank[q], a, s_loff, s_rpre);
+      }
+      if (a.packed_out) final_tile<true, true, true>(tile, nb_live - 1, r, n, now_ns, rv, nullptr, a.comp_sv, ring, out, a.counters, a.sv.run, a.sv.ever, base);
+      else final_tile<false, true, true>(tile, nb_live - 1, r, n, now_ns, rv, nullptr, a.comp_sv, ring, out, a.counters, a.sv.run, a.sv.ever, base);
     }
   } else if (a.solo) {
     // (tables too big for shared memory, or YDSCHED_FUSED_NOLITE: offsets scanned by the leader of E2)
@@ -493,10 +629,16 @@ __global__ void __launch_bounds__(1024, 1) k_fused_front(FusedArgs a) {
       loff = s_loff;
     }
     for (uint32_t tile = blockIdx.x; tile < nb_live; tile += G) {
+      uint32_t before = 0;  // (thread c) grants of class c in the tiles before this one, from the scanned counts
+      if (tid < ncls) {
+        const uint32_t* rrow = a.rank_cnt + tid * a.n_rtiles;
+        before = fused_class_grants(a, tid, rrow[tile] - rrow[0], loff[(tid + 1) * a.n_ltiles] - loff[tid * a.n_ltiles]);
+      }
+      const uint32_t base = fused_block_sum(before);
       const uint32_t q = tile * 1024 + tid;
       const uint32_t r = q < n ? fused_select(q, a, loff) : kResEnvNotFound;
-      if (a.packed_out) final_tile<true, true>(tile, nb_live - 1, r, n, now_ns, rv, a.look, a.comp_sv, ring, out, a.counters, a.sv.run, a.sv.ever);
-      else final_tile<false, true>(tile, nb_live - 1, r, n, now_ns, rv, a.look, a.comp_sv, ring, out, a.counters, a.sv.run, a.sv.ever);
+      if (a.packed_out) final_tile<true, true, true>(tile, nb_live - 1, r, n, now_ns, rv, nullptr, a.comp_sv, ring, out, a.counters, a.sv.run, a.sv.ever, base);
+      else final_tile<false, true, true>(tile, nb_live - 1, r, n, now_ns, rv, nullptr, a.comp_sv, ring, out, a.counters, a.sv.run, a.sv.ever, base);
     }
   } else {
     for (uint32_t tile = blockIdx.x; tile < nb_live; tile += G) {
@@ -510,11 +652,22 @@ __global__ void __launch_bounds__(1024, 1) k_fused_front(FusedArgs a) {
   }
   fused_stamp(a, 7);
   // ---- solo: the block that finishes last reports to the host and leaves the scratch as the next solve expects it ----
+  // A speculative solve resets the barrier words alone: the class table stays, and everything else it wrote is
+  // rewritten by the next one before it is read.  Any other solo solve keeps its class table when its class set is the
+  // one of the previous solve (the host speculates next), else it clears the table; the rest of the scratch is zeroed.
   if (a.solo && fused_done_last(a.bar)) {
-    fused_report(a, s_seq, a.counters->granted);
-    __syncthreads();  // (the report reads meta[], which lies in the region zeroed below)
-    for (uint32_t i = tid; i < kClsTableSize; i += 1024) a.clean_keys[i] = kClsEmpty;
-    for (uint32_t i = tid; i < a.clean_zero_vec; i += 1024) a.clean_zero[i] = make_uint4(0u, 0u, 0u, 0u);
+    if (a.spec) {
+      fused_report(a, s_seq, a.counters->granted);
+      if (tid < 3) a.bar[tid] = 0;
+    } else {
+      const unsigned long long fp = fused_classes_fp(a.clean_keys);
+      fused_report(a, s_seq, a.counters->granted, fp);
+      __syncthreads();  // (the report reads meta[], which lies in the region zeroed below)
+      uint32_t from = 0;
+      if (fp == s_kept_fp) from = kKeptClsWords / 4;
+      else for (uint32_t i = tid; i < kClsTableSize; i += 1024) a.clean_keys[i] = kClsEmpty;
+      for (uint32_t i = from + tid; i < a.clean_zero_vec; i += 1024) a.clean_zero[i] = make_uint4(0u, 0u, 0u, 0u);
+    }
     if (a.prof && tid == 0) a.prof[8] = fused_now();
   }
 }

@@ -22,33 +22,15 @@ namespace yd {
 
 constexpr int kRankTile = 1024;
 
-// One tile of 1024 requests (a block of 1024 threads).  Every (class, tile) cell of tile_cnt below cls_bound is written,
-// so tiles beyond the end of the queue must be run too (their cells are zero).
-__device__ __forceinline__ void rank_count_tile(uint32_t tile, const ReqView& reqs, uint32_t n,
-                                                const TopoView& t, const ClassTable& ct,
-                                                const uint32_t* __restrict__ comp_mode, uint32_t n_tiles,
-                                                uint32_t* __restrict__ rcls, uint32_t* __restrict__ rrank,
-                                                uint32_t* __restrict__ rself, uint32_t* __restrict__ tile_cnt) {
+// The FIFO rank of this thread's request (class `cls`, or kNone) among the requests of its class in tile `tile` (a block
+// of 1024 threads, thread = position in the tile), and the tile's per-class totals: every (class, tile) cell of tile_cnt
+// below cls_bound is written.
+__device__ __forceinline__ uint32_t rank_in_tile(uint32_t tile, uint32_t cls, const ClassTable& ct, uint32_t n_tiles,
+                                                 uint32_t* __restrict__ tile_cnt) {
   __shared__ uint16_t wc[32][kMaxClasses];
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   for (uint32_t i = tid; i < 32 * kMaxClasses / 2; i += kRankTile) reinterpret_cast<uint32_t*>(&wc[0][0])[i] = 0;
   __syncthreads();
-  const uint32_t q = tile * kRankTile + tid;
-  uint32_t cls = kNone, self = kNone;
-  if (q < n) {
-    uint32_t env, mv;
-    reqs.head(q, env, mv);
-    if (env < t.n_envs) {
-      const uint32_t comp = t.env_comp[env];
-      if (comp != kNone && comp_mode[comp] != 0) {  // data-parallel or merge: both need FIFO ranks
-        const uint32_t slot = cls_find(ct.keys, ((unsigned long long)env << 32) | mv);
-        if (slot != kNone) cls = ct.slot_cls[slot];
-        if (cls != kNone && comp_mode[comp] == 2 && (ct.comp_flags[comp] & 1u)) {
-          self = self_servant(t, reqs.ip(q), comp);
-        }
-      }
-    }
-  }
   const uint32_t peers = __match_any_sync(0xffffffffu, cls);
   const uint32_t wrank = __popc(peers & ((1u << lane) - 1));
   if (cls != kNone && wrank == 0) wc[warp][cls] = (uint16_t)__popc(peers);
@@ -66,12 +48,40 @@ __device__ __forceinline__ void rank_count_tile(uint32_t tile, const ReqView& re
   }
   if (tile == 0 && tid == 0) tile_cnt[ct.cls_bound * n_tiles] = 0;  // the scan's end cell
   __syncthreads();
+  const uint32_t rank = cls != kNone ? (uint32_t)wc[warp][cls] + wrank : 0u;
+  __syncthreads();  // (wc is reused when a block handles several tiles)
+  return rank;
+}
+
+// One tile of 1024 requests (a block of 1024 threads).  Every (class, tile) cell of tile_cnt below cls_bound is written,
+// so tiles beyond the end of the queue must be run too (their cells are zero).
+__device__ __forceinline__ void rank_count_tile(uint32_t tile, const ReqView& reqs, uint32_t n,
+                                                const TopoView& t, const ClassTable& ct,
+                                                const uint32_t* __restrict__ comp_mode, uint32_t n_tiles,
+                                                uint32_t* __restrict__ rcls, uint32_t* __restrict__ rrank,
+                                                uint32_t* __restrict__ rself, uint32_t* __restrict__ tile_cnt) {
+  const uint32_t q = tile * kRankTile + threadIdx.x;
+  uint32_t cls = kNone, self = kNone;
+  if (q < n) {
+    uint32_t env, mv;
+    reqs.head(q, env, mv);
+    if (env < t.n_envs) {
+      const uint32_t comp = t.env_comp[env];
+      if (comp != kNone && comp_mode[comp] != 0) {  // data-parallel or merge: both need FIFO ranks
+        const uint32_t slot = cls_find(ct.keys, ((unsigned long long)env << 32) | mv);
+        if (slot != kNone) cls = ct.slot_cls[slot];
+        if (cls != kNone && comp_mode[comp] == 2 && (ct.comp_flags[comp] & 1u)) {
+          self = self_servant(t, reqs.ip(q), comp);
+        }
+      }
+    }
+  }
+  const uint32_t rank = rank_in_tile(tile, cls, ct, n_tiles, tile_cnt);
   if (q < n) {
     rcls[q] = cls;
-    rrank[q] = cls != kNone ? (uint32_t)wc[warp][cls] + wrank : 0u;
+    rrank[q] = rank;
     rself[q] = self;
   }
-  __syncthreads();  // (wc is reused when a block handles several tiles)
 }
 
 __global__ void __launch_bounds__(kRankTile) k_rank_count(const yd_task_req* __restrict__ reqs,

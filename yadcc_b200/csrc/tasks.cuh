@@ -140,15 +140,15 @@ __global__ void __launch_bounds__(1024) k_final_write(const uint32_t* __restrict
 // final_tile: tile `vb` of 1024 requests, r = the solver's verdict for request vb * 1024 + tid (kResEnvNotFound beyond
 // the queue's end).  Tiles below vb must be running or done.  kPacked: 8-byte grants {servant_index, status << 30 |
 // FIFO ordinal of the grant}, see yd_grant8 in ydsched.h.
-// kPos: r is already a registry position (else an index into comp_sv).  kFlat: the tiles run side by side (fused kernel,
-// one tile per resident block): every predecessor's COUNT is fetched, 128 per round trip, instead of walking back to
-// the nearest published prefix -- the last tile finishes one L2 round trip after the slowest predecessor has counted.
-template <bool kPacked, bool kPos = false, bool kFlat = false>
+// kPos: r is already a registry position (else an index into comp_sv).  kBase: the caller knows the grants of the tiles
+// before this one (`base`; the fused solo kernel derives it from its per-class counts): no look-back, `look` is unused.
+template <bool kPacked, bool kPos = false, bool kBase = false>
 __device__ __forceinline__ void final_tile(uint32_t vb, uint32_t last_vb, uint32_t r, uint32_t n, long long now_ns,
                                            const ReqView& reqs, unsigned long long* __restrict__ look,
                                            const uint32_t* __restrict__ comp_sv, const TaskRing& ring,
                                            void* __restrict__ out, Counters* __restrict__ counters,
-                                           uint32_t* __restrict__ run, unsigned long long* __restrict__ ever) {
+                                           uint32_t* __restrict__ run, unsigned long long* __restrict__ ever,
+                                           unsigned long long base = 0) {
   __shared__ uint32_t warp_cnt[32];
   __shared__ unsigned long long s_excl;
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -161,28 +161,9 @@ __device__ __forceinline__ void final_tile(uint32_t vb, uint32_t last_vb, uint32
   if (warp == 0) {
     const uint32_t mine = __reduce_add_sync(0xffffffffu, warp_cnt[lane]);
     volatile unsigned long long* vl = look;
-    if (lane == 0) { __threadfence(); vl[vb] = (1ull << 62) | mine; }
-    unsigned long long excl = 0;
-    int at = kFlat ? -1 : (int)vb - 1;
-    if (kFlat) {
-      for (uint32_t base = 0; base < vb; base += 128) {
-        unsigned long long v[4];
-        bool missing;
-        do {
-          missing = false;
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const uint32_t idx = base + k * 32 + lane;
-            v[k] = idx < vb ? vl[idx] : (1ull << 62);
-            missing |= (v[k] >> 62) == 0;
-          }
-        } while (__any_sync(0xffffffffu, missing));
-#pragma unroll
-        for (int k = 0; k < 4; ++k) excl += v[k] & ((1ull << 62) - 1);
-      }
-#pragma unroll
-      for (int d = 16; d; d >>= 1) excl += __shfl_xor_sync(0xffffffffu, excl, d);
-    }
+    if (!kBase && lane == 0) { __threadfence(); vl[vb] = (1ull << 62) | mine; }
+    unsigned long long excl = kBase ? base : 0ull;
+    int at = kBase ? -1 : (int)vb - 1;
     while (at >= 0) {
       const int idx = at - (int)lane;
       unsigned long long v;
@@ -206,7 +187,7 @@ __device__ __forceinline__ void final_tile(uint32_t vb, uint32_t last_vb, uint32
       at -= 32;
     }
     if (lane == 0) {
-      if (!kFlat) {  // (flat: the word keeps this tile's COUNT, which is what the later tiles add up)
+      if (!kBase) {
         __threadfence();
         vl[vb] = (2ull << 62) | (excl + mine);
       }

@@ -211,7 +211,16 @@ struct yd_sched {
     bool operator==(const CleanSig& o) const { return gen == o.gen && z_cls_off == o.z_cls_off && z_bytes == o.z_bytes && res_words == o.res_words && zero == o.zero && res == o.res; } };
   CleanSig clean_sig;
   bool clean_valid = false;
-  bool fused_lite = true;      // YDSCHED_FUSED_NOLITE: the solo kernel's second barrier keeps its leader scans
+  // A solo solve that finds the class set of the previous one keeps its class table (fused.cuh); the next solo solve
+  // then runs the speculative variant on it, while the buffers, the topology and the class bound are those it was built
+  // with.  kept_fp = the class-set fingerprint of the last non-speculative solo solve (0: none -- nothing to compare
+  // with, as after a speculative solve missed): speculation resumes only after two such solves in a row agree.
+  struct KeptSig { CleanSig clean; unsigned long long topo_gen = 0; uint32_t cls_bound = 0;
+    bool operator==(const KeptSig& o) const { return clean == o.clean && topo_gen == o.topo_gen && cls_bound == o.cls_bound; } };
+  KeptSig kept_sig;
+  bool kept_valid = false;
+  unsigned long long kept_fp = 0;
+  bool fused_lite = true;     // YDSCHED_FUSED_NOLITE: the solo kernel's second barrier keeps its leader scans
   bool zero_copy = true;       // YDSCHED_NO_ZEROCOPY: page-locked caller arrays are copied like pageable ones
   bool fused_prof = false;     // YDSCHED_FUSED_PROF: phase stamps of the fused kernel, printed after every solve
   DevBuf d_fused_prof;
@@ -1095,7 +1104,7 @@ constexpr size_t kFusedLoffCacheWords = 16384;  // 64 KB of dynamic shared memor
 // The fused front (fused.cuh): classes, ranks, lists and the data-parallel verdicts in ONE persistent launch on `st`;
 // `solo`: grants, task ids and leases too (batches made of data-parallel components only), else the coupled solvers
 // follow.  Needs the kept slot order.
-uint32_t LaunchFused(yd_sched* s, uint32_t N, size_t slot_b, bool capturing, bool solo, bool packed_in, bool packed_out) {
+uint32_t LaunchFused(yd_sched* s, uint32_t N, size_t slot_b, bool capturing, bool solo, bool spec, bool packed_in, bool packed_out) {
   cudaStream_t st = s->st;
   uint32_t launches = 0;
   const uint32_t n_tiles = (uint32_t)((slot_b + yd::kListTile - 1) / yd::kListTile);
@@ -1138,7 +1147,6 @@ uint32_t LaunchFused(yd_sched* s, uint32_t N, size_t slot_b, bool capturing, boo
   a.bar = reinterpret_cast<uint32_t*>(static_cast<char*>(s->d_zero.p) + s->z_fbar_off);
   a.solo = solo ? 1u : 0u;
   a.packed_out = packed_out ? 1u : 0u;
-  a.look = reinterpret_cast<unsigned long long*>(static_cast<char*>(s->d_zero.p) + s->z_final_off);
   a.comp_sv = s->d_comp_sv.as<uint32_t>();
   a.ring = s->ring();
   a.out = packed_out ? s->d_out8.p : s->d_out.p;
@@ -1152,6 +1160,7 @@ uint32_t LaunchFused(yd_sched* s, uint32_t N, size_t slot_b, bool capturing, boo
   const size_t dyn = solo && cells <= kFusedLoffCacheWords ? cells * 4 : 0;
   a.loff_cache_words = (uint32_t)(dyn / 4);
   a.lite = s->fused_lite ? 1u : 0u;
+  a.spec = spec ? 1u : 0u;
   yd::k_fused_front<<<grid, 1024, dyn, st>>>(a);
   s->last_fused = a;
   s->last_fused_grid = grid;
@@ -1178,7 +1187,8 @@ uint64_t NextPow2(uint64_t v, uint64_t lo) {
 
 // Everything between the request upload and the grant download, for size class
 // (Nb, slot_b): the sequence that is captured into a CUDA graph.
-// variant: 0 = the kernel-by-kernel pipeline, 1 = fused front + coupled solvers + final, 2 = fused front alone (solo).
+// variant: 0 = the kernel-by-kernel pipeline, 1 = fused front + coupled solvers + final, 2 = fused front alone (solo),
+// 3 = the same on a clean scratch (no memset nodes), 4 = solo and speculative on the kept class table (no memsets).
 // packed bit 0: the upload is 16-byte records in d_reqs16; bit 1: the download is 8-byte grants from d_out8.
 uint32_t EnqueueSolve(yd_sched* s, uint32_t Nb, size_t slot_b, uint32_t solver, bool record_events, bool capturing,
                       uint32_t variant = 0, uint32_t packed = 0) {
@@ -1215,7 +1225,7 @@ uint32_t EnqueueSolve(yd_sched* s, uint32_t Nb, size_t slot_b, uint32_t solver, 
   }
   if (have_work && solver == 2) {
     if (record_events) YD_CUDA_CHECK(cudaEventRecord(s->ev[2], st));
-    if (variant) launches += LaunchFused(s, Nb, slot_b, capturing, variant >= 2, packed_in, packed_out);
+    if (variant) launches += LaunchFused(s, Nb, slot_b, capturing, variant >= 2, variant == 4, packed_in, packed_out);
     else launches += LaunchStream(s, Nb, slot_b, capturing);
     abort_flag = MakeClassTable(s).meta + 1;
   } else {
@@ -1503,9 +1513,19 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
     if (variant == 2) {
       if (solver == 2) PrepareStreamBuffers(s, Nb, slot_b);  // (fixes the scratch layout the signature describes)
       sig_now = yd_sched::CleanSig{g_buf_generation, s->z_cls_off, s->z_bytes, s->res_words, s->d_zero.p, s->d_res.p};
-      if (s->clean_valid && s->clean_sig == sig_now) variant = 3;  // no memset nodes: the graph is the kernel alone
+      // speculative (fused.cuh): the kept class table is the one these buffers, this topology and this class bound
+      // had; every block holds at most two request tiles (their classes and ranks stay in registers) and the lists'
+      // offsets fit in shared memory (the selection without leader scans)
+      const size_t lcells = size_t(s->cls_bound) * ((slot_b + yd::kListTile - 1) / yd::kListTile + 1) + 1;
+      if (s->kept_valid && s->kept_sig == yd_sched::KeptSig{sig_now, s->topo_gen, s->cls_bound} && s->fused_lite &&
+          lcells <= kFusedLoffCacheWords && (Nb + yd::kRankTile - 1) / yd::kRankTile <= 2 * s->fused_grid) {
+        variant = 4;  // the graph is the kernel alone
+      } else if (s->clean_valid && s->clean_sig == sig_now) {
+        variant = 3;  // no memset nodes: the graph is the kernel alone
+      }
     }
     s->clean_valid = false;  // (whatever runs now dirties the scratch; a completed solo solve says otherwise below)
+    if (variant != 4) s->kept_valid = false;  // (any other solve rebuilds or clears the class table)
     // (a staged solve -- no request array in this call -- leaves its grants in HBM and copies them afterwards, so that
     // the device-side events around it time the solve alone)
     const bool zc_in = variant >= 1 && in_dev, zc_out = variant >= 2 && out_dev && in_host;
@@ -1515,6 +1535,7 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
     s->fsc.zc_in = zc_in ? in_dev : nullptr;
     s->fsc.zc_out = zc_out ? out_dev : nullptr;
     s->fsc.seq += 1;
+    s->fsc.kept_fp = s->kept_fp;
     *s->h_fsc.as<yd::FusedScalars>() = s->fsc;
     s->h_fio->done_seq = 0;
     if (s->use_graphs) {
@@ -1609,7 +1630,16 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
       s->h_counters.as<Counters>()->granted = s->h_fio->granted;
     }
     if (s->dump_env && solver == 2 && S && s->n_comps) DumpStreamState(s, Nb, slot_b);
-    if (s->fused_prof && variant) {
+    if (s->fused_prof && variant == 4) {
+      unsigned long long t[9];
+      YD_CUDA_CHECK(cudaMemcpy(t, s->d_fused_prof.p, sizeof t, cudaMemcpyDeviceToHost));
+      if (s->h_meta.as<uint32_t>()[1] == yd::kFlagSpecMiss) {  // (no phase B)
+        fprintf(stderr, "ydsched: fused variant 4 (speculative) n %u ns: A %llu barrier %llu missed\n", N, t[1] - t[0], t[2] - t[1]);
+      } else {
+        fprintf(stderr, "ydsched: fused variant 4 (speculative) n %u ns: A %llu barrier %llu B %llu total %llu (+tail %lld)\n", N,
+                t[1] - t[0], t[2] - t[1], t[7] - t[2], t[7] - t[0], (long long)(t[8] - t[7]));
+      }
+    } else if (s->fused_prof && variant) {
       unsigned long long t[9];
       YD_CUDA_CHECK(cudaMemcpy(t, s->d_fused_prof.p, sizeof t, cudaMemcpyDeviceToHost));
       fprintf(stderr, "ydsched: fused variant %u n %u ns: P1 %llu E1 %llu P3 %llu E2 %llu P5 %llu B3 %llu P6 %llu total %llu (+report/clean %lld)\n", variant, N,
@@ -1618,7 +1648,14 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
     if (solver == 2 && S && s->n_comps && s->h_meta.as<uint32_t>()[1] != 0) {
       // Nothing was decided (the stream solver and the final kernels all stood down).
       const uint32_t flag = s->h_meta.as<uint32_t>()[1], ncls = s->h_meta.as<uint32_t>()[0];
-      if (flag == 4) {  // the solo kernel met a component it cannot decide: the general sequence, now and next time
+      if (flag == yd::kFlagSpecMiss) {
+        // the kept class table could not decide the batch and the kernel left the scratch clean: replay without
+        // speculation (which builds the table again), and speculate again only once two solves agree on the class set
+        s->kept_valid = false;
+        s->kept_fp = 0;
+        s->clean_sig = sig_now;
+        s->clean_valid = true;
+      } else if (flag == 4) {  // the solo kernel met a component it cannot decide: the general sequence, now and next time
         s->solo_hint = false;
       } else if (flag == 2 && grow_attempts++ < 3 && s->cls_bound < yd::kMaxClasses) {  // more lists than provisioned: grow and go again
         // one list per class plus one pseudo-class list per merge-mode component
@@ -1657,11 +1694,20 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
       continue;
     }
     if (variant == 1) s->solo_hint = s->h_meta.as<uint32_t>()[4] == 0;  // back to one launch when nothing is coupled any more
-    if (variant >= 2) {  // completed: the kernel's last block has re-initialised the scratch
+    if (variant == 2 || variant == 3) {
+      // completed: the kernel's last block has kept the class table (same class set as the previous such solve) or
+      // cleared it, and re-initialised the rest of the scratch
       if (variant == 2) sig_now = yd_sched::CleanSig{g_buf_generation, s->z_cls_off, s->z_bytes, s->res_words, s->d_zero.p, s->d_res.p};
-      s->clean_sig = sig_now;
-      s->clean_valid = true;
-    }
+      const unsigned long long fp = s->h_fio->classes_fp;
+      if (fp == s->kept_fp) {
+        s->kept_sig = yd_sched::KeptSig{sig_now, s->topo_gen, s->cls_bound};
+        s->kept_valid = true;
+      } else {
+        s->clean_sig = sig_now;
+        s->clean_valid = true;
+      }
+      s->kept_fp = fp;
+    }  // (variant 4 completed: the kept table stays valid)
     break;
   }
   const Counters* c = s->h_counters.as<Counters>();

@@ -1419,6 +1419,7 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
     s->stats.h2d_bytes = 0;  // the requests are kernel arguments
     s->stats.d2h_bytes = size_t(N) * sizeof(yd_grant) + 8;  // written by the kernel into pinned host memory
     s->have_stats = true;
+    if (s->debug_env) fprintf(stderr, "ydsched: solve n %u tiny 1 solver 3 solve_ms %.3f\n", N, ms);
     return;
   }
 
@@ -1497,13 +1498,14 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
   bool graphed = false;
   const uint32_t merge_rounds_cfg = s->merge_rounds, force_stream_cfg = s->force_stream;
   int merge_retry = 0, grow_attempts = 0;
+  uint32_t variant = 0;
   for (;;) {
     memset(s->h_meta.p, 0, 32);
     graphed = false;
     // The fused front kernel takes batches in the latency-bound regime whose (class, tile) count matrices one block
     // scans in a few rounds; it needs the kept slot order.  solo = it also writes the grants (no coupled component
     // had requests last time; if one has now, the kernel raises flag 4 and the batch is replayed with variant 1).
-    uint32_t variant = 0;
+    variant = 0;
     if (s->fused_cfg && s->fused_grid && s->solver_pref == 0 && solver == 2 && want_static && S && s->n_comps && Nb <= s->fused_max_nb &&
         size_t(s->cls_bound) * ((Nb + yd::kRankTile - 1) / yd::kRankTile) <= 32768 &&
         size_t(s->cls_bound) * ((slot_b + yd::kListTile - 1) / yd::kListTile) <= 32768) {
@@ -1732,8 +1734,16 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
             hp[1] - hp[0], hp[2] - hp[1], hp[3] - hp[2], hp[4] - hp[3], hp[5] - hp[4], hp[6] - hp[5], hp[7] - hp[6], hp[7] - hp[0]);
   }
   if (s->debug_env) {
-    fprintf(stderr, "ydsched: solver %u graph %d merge_rounds %llu merge_chunks %llu walks %llu windows %llu solve_ms %.3f\n",
-            solver, (int)graphed, c->pad[0], c->pad[1], c->pad[2], c->pad[3], stt.solve_ms);
+    // which path the solve took (the last attempt, after any stand-down): `final` 0 = the solo kernel wrote the grants,
+    // 1 = k_final_fused, 3 = k_final_count / k_final_scan / k_final_write
+    const bool have_work = S && s->n_comps;
+    const uint32_t final_path = (variant >= 2 && have_work && solver == 2) ? 0u : (solver == 2 && have_work && nb <= 2048) ? 1u : 3u;
+    fprintf(stderr, "ydsched: solve n %u tiny 0 variant %u order_static %d wide %d Nb %u slot_b %zu cls_bound %u final %u "
+            "emask %d max_comp %zu solver %u graph %d merge_rounds %llu merge_chunks %llu walks %llu windows %llu "
+            "solve_ms %.3f\n",
+            N, variant, (int)(solver == 2 && s->order_static), (int)s->wide, Nb, slot_b, s->cls_bound, final_path,
+            (int)s->emask_ok, (size_t)s->max_comp_servants, solver, (int)graphed, c->pad[0], c->pad[1], c->pad[2],
+            c->pad[3], stt.solve_ms);
   }
 }
 }  // namespace

@@ -30,6 +30,14 @@ def test_fuzz_port_equals_reference(make_dispatcher, seed):
                            lambda d: S.fuzz_stream(d, seed, n_servants=8 + seed % 30, wide=(seed % 5 == 0)))
 
 
+@pytest.mark.parametrize("seed", [0, 1, 2, 3, 5, 11])
+def test_solo_stream_port_equals_reference(make_dispatcher, seed):
+    """The solo-path streams of tests/test_solo_state.py: version gating, servant churn, shared hosts, zombies, the
+    lease ring past 2^17 ids (seeds 0, 3) with a pinned window (seed 0) -- the reference's behaviour, not the
+    restatement's."""
+    _port_equals_reference(make_dispatcher, f"solo-{seed}", lambda d: S.solo_stream(d, seed))
+
+
 @pytest.mark.parametrize("name", ["cfg1", "cfg2-mod-small", "cfg2-random-small", "cfg3-small"])
 def test_configs_port_equals_reference(make_dispatcher, name):
     _port_equals_reference(make_dispatcher, f"config-{name}", lambda d: S.named_stream(name, d))

@@ -12,6 +12,7 @@ import pytest
 
 import key_cases as K
 from conftest import REF_LIB
+from solve_lines import solves as _solves
 from yadcc_b200 import PRIORITY_DEDICATED, PRIORITY_USER, STATUS_GRANTED, Servant
 from yadcc_b200 import streams as S
 from yadcc_b200._abi import STATUS_ENVIRONMENT_NOT_FOUND
@@ -22,16 +23,6 @@ GiB = 1 << 30
 STATIC_SLOT_LIMIT = 1 << 26  # kStaticSlotLimit
 THREE_PASS_N = (1 << 21) + 1  # nb = NextPow2(N) / 1024 > 2048
 FUSED_MAX_N = 262144          # fused_max_nb
-
-
-def _solves(err: str) -> list[dict]:
-    """The `key value` pairs of every YDSCHED_DEBUG solve line."""
-    out = []
-    for line in err.splitlines():
-        if line.startswith("ydsched: solve n "):
-            t = line[len("ydsched: solve "):].split()
-            out.append({k: float(v) if "." in v else int(v) for k, v in zip(t[::2], t[1::2])})
-    return out
 
 
 def _checkers():

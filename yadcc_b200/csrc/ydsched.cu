@@ -1419,7 +1419,10 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
     s->stats.h2d_bytes = 0;  // the requests are kernel arguments
     s->stats.d2h_bytes = size_t(N) * sizeof(yd_grant) + 8;  // written by the kernel into pinned host memory
     s->have_stats = true;
-    if (s->debug_env) fprintf(stderr, "ydsched: solve n %u tiny 1 solver 3 solve_ms %.3f\n", N, ms);
+    if (s->debug_env) {
+      fprintf(stderr, "ydsched: solve n %u tiny 1 solver 3 spec 0 ring_cap %llu ring_lo %llu solve_ms %.3f\n", N,
+              (unsigned long long)s->ring_cap, (unsigned long long)s->lo, ms);
+    }
     return;
   }
 
@@ -1499,6 +1502,7 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
   const uint32_t merge_rounds_cfg = s->merge_rounds, force_stream_cfg = s->force_stream;
   int merge_retry = 0, grow_attempts = 0;
   uint32_t variant = 0;
+  uint32_t spec = 0;  // the speculative variant: 0 not tried, 1 decided the batch, 2 missed (the batch was replayed)
   for (;;) {
     memset(s->h_meta.p, 0, 32);
     graphed = false;
@@ -1653,6 +1657,7 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
       if (flag == yd::kFlagSpecMiss) {
         // the kept class table could not decide the batch and the kernel left the scratch clean: replay without
         // speculation (which builds the table again), and speculate again only once two solves agree on the class set
+        spec = 2;
         s->kept_valid = false;
         s->kept_fp = 0;
         s->clean_sig = sig_now;
@@ -1710,6 +1715,7 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
       }
       s->kept_fp = fp;
     }  // (variant 4 completed: the kept table stays valid)
+    if (variant == 4) spec = 1;
     break;
   }
   const Counters* c = s->h_counters.as<Counters>();
@@ -1735,15 +1741,16 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
   }
   if (s->debug_env) {
     // which path the solve took (the last attempt, after any stand-down): `final` 0 = the solo kernel wrote the grants,
-    // 1 = k_final_fused, 3 = k_final_count / k_final_scan / k_final_write
+    // 1 = k_final_fused, 3 = k_final_count / k_final_scan / k_final_write; `spec` over all attempts; the lease ring
+    // (`ring_lo` = the first live id) as the solve found it
     const bool have_work = S && s->n_comps;
     const uint32_t final_path = (variant >= 2 && have_work && solver == 2) ? 0u : (solver == 2 && have_work && nb <= 2048) ? 1u : 3u;
     fprintf(stderr, "ydsched: solve n %u tiny 0 variant %u order_static %d wide %d Nb %u slot_b %zu cls_bound %u final %u "
             "emask %d max_comp %zu solver %u graph %d merge_rounds %llu merge_chunks %llu walks %llu windows %llu "
-            "solve_ms %.3f\n",
+            "spec %u ring_cap %llu ring_lo %llu solve_ms %.3f\n",
             N, variant, (int)(solver == 2 && s->order_static), (int)s->wide, Nb, slot_b, s->cls_bound, final_path,
             (int)s->emask_ok, (size_t)s->max_comp_servants, solver, (int)graphed, c->pad[0], c->pad[1], c->pad[2],
-            c->pad[3], stt.solve_ms);
+            c->pad[3], spec, (unsigned long long)s->ring_cap, (unsigned long long)s->lo, stt.solve_ms);
   }
 }
 }  // namespace

@@ -12,9 +12,11 @@ Event kinds (tuples, first element is the kind):
   ("solve", now)                              offer the whole pending queue in order
                                               (zero-wait); Timeout requests stay
                                               pending, everything else leaves
-  ("wait", now, REQ array)                    one-shot batch, no pending queue
+  ("wait", now, REQ array | f(dispatcher))    one-shot batch, no pending queue (f builds it when the event runs:
+                                              requestor IPs interned between solves)
   ("free", ids)                               FreeTask per id
-  ("free_frac", seed, frac)                   free a seeded subset of outstanding grants
+  ("free_frac", seed, frac[, spare])          free a seeded subset of outstanding grants (except those on the
+                                              servant indices in `spare`)
   ("keepalive", now, ids | None, expires_in)  KeepTaskAlive (None = all outstanding)
   ("tick", now)                               OnExpirationTimer
   ("notify", location, [(servant_task_id, grant_id, digest)])
@@ -160,17 +162,19 @@ class Replayer:
                 self.pending = self.pending[g["status"] == STATUS_TIMEOUT]
                 trace.append(g)
             elif kind == "wait":
-                trace.append(self._wait(ev[1], ev[2]))
+                trace.append(self._wait(ev[1], ev[2](d) if callable(ev[2]) else ev[2]))
             elif kind == "free":
                 ids = np.asarray(ev[1], dtype=np.uint64)
                 d.free_tasks(ids)
                 for i in ids.tolist():
                     self.outstanding.pop(i, None)
             elif kind == "free_frac":
-                _, seed, frac = ev
+                _, seed, frac, *spare = ev
                 ids = np.fromiter(sorted(self.outstanding), dtype=np.uint64, count=len(self.outstanding))
                 rng = np.random.default_rng(seed)
                 pick = ids[rng.random(len(ids)) < frac]
+                if spare:
+                    pick = pick[np.asarray([self.outstanding[i] not in spare[0] for i in pick.tolist()], dtype=bool)]
                 d.free_tasks(pick)
                 for i in pick.tolist():
                     self.outstanding.pop(i, None)
@@ -539,6 +543,341 @@ def fuzz_stream(d: TaskDispatcher, seed: int, n_servants: int = 24, n_events: in
             ev.append(("state",))
     ev.append(("state",))
     return Stream(f"fuzz-{seed}", ev, {"seed": seed, "servants": n_servants})
+
+
+# ---------------------------------------------------------------------------
+# solo: the one-launch solve's state from one call to the next
+# ---------------------------------------------------------------------------
+
+# What ends a steady stretch of `solo_stream`, and the path of the batch it bears on (fused.cuh, ydsched.cu WaitImpl):
+#   hit        the speculative solve decides it on the kept class table and the kept slot order
+#   rebuild    the speculative solve decides it, after the slot order was rebuilt
+#   replay     the speculative solve misses; the batch is replayed on the clean scratch (variant 3)
+#   standdown  the speculative solve misses; the replay stands down (flag 4) to the general sequence
+#   fresh      a new topology: a full solo solve, no speculation
+#   nospec     the batch cannot speculate
+SOLO_MENU = {
+    "version-up": "hit", "version-down": "hit", "version-drop-last": "hit",
+    "load": "rebuild", "nproc": "rebuild", "max-tasks-0": "rebuild", "max-tasks-back": "rebuild",
+    "low-memory": "rebuild", "priority": "rebuild",
+    "keepalive": "hit", "free-unknown": "hit", "notify-bogus": "hit", "tick-leases": "hit", "tiny": "hit",
+    "new-min-version": "replay", "new-digest": "replay",
+    "self": "standdown", "two-min-versions": "standdown",
+    "digest-set": "fresh", "new-servant": "fresh", "servant-expiry": "fresh",
+    "size-class": "nospec", "class-bound": "nospec",
+}
+# perturbations that are a batch themselves (the others are events before the next stretch's first batch)
+_SOLO_BATCHES = ("new-min-version", "new-digest", "self", "two-min-versions", "size-class", "class-bound")
+_SIZE_CLASSES = {1024: (9, 1024), 2048: (1025, 2048), 4096: (2049, 3000)}  # Nb = NextPow2(n, 1024): n range
+
+
+def _np2(x: int, lo: int) -> int:
+    return max(lo, 1 << (max(x, 1) - 1).bit_length())
+
+
+def solo_stream(d: TaskDispatcher, seed: int, *, wrap: bool | None = None, grow: bool | None = None) -> Stream:
+    """Steady stretches of data-parallel batches (every servant holds one digest, one min_version per digest), each
+    ended by one perturbation from SOLO_MENU, so that the one-launch solve's kept state -- slot order, class table,
+    clean scratch, solo hint, servant facts on the device, lease ring -- is used and invalidated in every way a call
+    sequence can.  meta["checks"] lists (batch, perturbation, expected path); a batch is the index of a "wait" event.
+
+    `wrap` (default: every third seed): batches of 2049-3000 requests over a larger cluster, most grants freed after
+    each, until more than 2^17 task ids were handed out -- the lease ring's live window crosses the ring's end.
+    `grow` (default: every sixth seed): from about 20 000 ids on, the grants on servants 0 and 1 are neither freed
+    nor swept, for 90 000 requests: the live window outgrows the ring while it straddles the ring's end.
+    """
+    rng = np.random.default_rng(seed)
+    wrap = seed % 3 == 0 if wrap is None else wrap
+    grow = seed % 6 == 0 if grow is None else grow
+    K = 4 + seed % 9 if grow else 2 + seed % 11
+    n_servants = int(rng.integers(400, 601)) if wrap else int(rng.integers(64, 301))
+    dgs = [f"{0x50100000 + (seed << 8) + k:064x}" for k in range(K)]
+    env = np.asarray([d.intern_env(x) for x in dgs], dtype=np.uint32)
+    unknown = np.asarray([d.intern_env(f"{0x5010dead + (seed << 8) + k:064x}") for k in range(2)], dtype=np.uint32)
+    pins = (0, 1) if grow else ()
+    net = 80 + seed % 100
+    if seed % 4 == 1:  # shared hosts: three servants per IP, in three components (i mod K differ)
+        host = lambda i: f"10.{net}.{(i // 3) >> 8}.{(i // 3) & 255}"  # noqa: E731
+    else:
+        host = lambda i: f"10.{net}.{i >> 8}.{i & 255}"  # noqa: E731
+
+    def new_servant(i: int, digest: int) -> Servant:
+        envs = [dgs[digest]] * (2 if rng.random() < 0.08 else 1)  # (a duplicate digest in one heartbeat)
+        if i in pins:  # healthy, so that they hold grants from the first batch of the pinned window on
+            return Servant(f"{host(i)}:{8000 + i}", None, envs, 9, 128, 0, 64 * GiB, 40 * GiB, 120, _abi.PRIORITY_USER)
+        nproc = int(rng.choice([32, 64, 96, 128]))
+        dedicated = rng.random() < 0.15
+        if dedicated and rng.random() < 0.5:
+            nproc += 1  # odd: the dedicated tier's edge 2r < P falls between two slots
+        mt = nproc * 95 // 100 if dedicated else nproc * 40 // 100
+        if rng.random() < 0.05:
+            mt = 0
+        if dedicated:
+            load = nproc // 2 + int(rng.integers(-1, 2))
+        elif rng.random() < 0.06:
+            load = nproc + int(rng.integers(1, 8))  # load above nproc
+        else:
+            load = int(rng.integers(0, nproc + 1)) if rng.random() < 0.4 else int(rng.integers(0, 4))
+        return Servant(f"{host(i)}:{8000 + i}", None, envs, int(rng.choice([-1, 6, 7, 8, 9, 9])), nproc, load,
+                       64 * GiB, 5 * GiB if rng.random() < 0.15 else 40 * GiB, mt,
+                       _abi.PRIORITY_DEDICATED if dedicated else _abi.PRIORITY_USER)
+
+    # the registry as the scheduler keeps it, in position order (expired servants erased): (creation index, facts)
+    sv: list[tuple[int, Servant]] = [(i, new_servant(i, i % K)) for i in range(n_servants)]
+    made = n_servants
+    ev: list = [("hb", 0.0, s, 1e6) for _, s in sv]
+    # The id staging of FreeTask / KeepTaskAlive at its largest size first: a device buffer that grows drops the kept
+    # class table (CleanSig holds the buffer generation), which would blur which event a path follows.
+    bogus = np.arange(1 << 40, (1 << 40) + (1 << 17), dtype=np.uint64)
+    ev += [("free", bogus), ("keepalive", 0.0, bogus, 1.0)]
+    clients = np.asarray([d.intern_ip(f"172.30.{seed % 250}.{k}") for k in range(64)], dtype=np.uint32)
+    late_names: list[str] = []  # client IPs that the batches intern themselves, after earlier solves
+    zero = K - 1  # min_version 10, above every servant: EnvironmentNotFound with cls_nelig == 0
+    mv = {k: int(rng.choice([7, 8, 9])) for k in range(K)}
+    mv[zero] = 10
+    classes = sorted({k for k in range(K - 1) if rng.random() < 0.7 or k < len(pins)} | {zero})
+    if len(classes) == K and K > 2:
+        classes.remove(K - 2)  # a held digest left out: the "new-digest" batch adds it
+    size = 4096 if wrap else int(rng.choice(list(_SIZE_CLASSES)))
+    st = {"now": 0.001, "issued": 0, "waits": 0, "pinned": False}
+    checks: list = []
+    saved_mt: list = []  # (location, max_tasks) of servants set to max_tasks 0
+    dropped: list = []   # digests whose eligible servants all went below its min_version
+
+    def digest_of(s: Servant) -> int:
+        return dgs.index(s.environments[0])
+
+    def holders(k: int) -> list[int]:
+        return [p for p, (_, s) in enumerate(sv) if digest_of(s) == k]
+
+    def movers() -> list[int]:  # positions whose servant may change or leave (pins stay as they are)
+        return [p for p, (i, _) in enumerate(sv) if i not in pins]
+
+    def pick(xs):
+        return xs[int(rng.integers(0, len(xs)))]
+
+    def hb(p: int, s: Servant, expires: float = 1e6) -> None:
+        sv[p] = (sv[p][0], s)
+        ev.append(("hb", st["now"], s, expires))
+
+    def slot_b() -> int:
+        return _np2(sum(min(s.num_processors, s.max_tasks) + 1 for _, s in sv), 4096)
+
+    def between() -> None:  # after every batch: frees (not of the pinned grants), maybe a zombie sweep, a tick, state
+        frac = 0.9 if wrap else 0.5
+        ev.append(("free_frac", int(rng.integers(1 << 30)), frac) + ((pins,) if st["pinned"] else ()))
+        if rng.random() < 0.3:
+            ev.append(("notify_own", pick(movers()), int(rng.integers(1 << 30)), []))
+        st["now"] += 0.003
+        ev.append(("tick", st["now"]))
+        ev.append(("state",))
+        st["now"] += 0.003
+
+    def batch(n: int, *, k=None, m=None, self_req: bool = False) -> None:
+        """n requests over the stretch's digests (each at least once), 1 % unknown digests; requestors are clients,
+        servants of other components, clients interned by this very batch, and (self_req) servants of their own."""
+        if k is None:
+            k = np.asarray(classes)[rng.integers(0, len(classes), n)]
+            k[: min(n, len(classes))] = classes[: n]
+        if m is None:
+            m = np.asarray([mv[int(x)] for x in k], dtype=np.uint32)
+        e = env[k]
+        unk = rng.random(n) < 0.01
+        unk[: len(classes) + 1] = False
+        e[unk] = unknown[rng.integers(0, 2, int(unk.sum()))]
+        by_host: dict[str, set[int]] = {}
+        for _, s in sv:
+            by_host.setdefault(s.observed_location.split(":")[0], set()).add(digest_of(s))
+        names = sorted(by_host)
+        hosts = {(c, o): [h for h in names if (c in by_host[h]) == o] for c in set(k.tolist()) for o in (False, True)}
+        ips = clients[rng.integers(0, len(clients), n)]
+        u = rng.random(n)
+        own = (u < 0.1) if self_req else np.zeros(n, dtype=bool)
+        own[0] = self_req
+        for q in np.nonzero((u < 0.35) | own)[0].tolist():
+            cand = hosts[int(k[q]), bool(own[q])]
+            if cand:
+                ips[q] = d.intern_ip(pick(cand))
+        r = _requests(d, e, ips, m, expires_in_s=15.0, prefetch=rng.random(n) < 0.2)
+        r["expires_in_ns"][rng.random(n) < 0.3] = 4_000_000  # short leases: zombies by the next tick
+        late = np.nonzero((u > 0.93) & ~own)[0]
+        if len(late):
+            late_names.extend(f"192.168.{seed % 250}.{len(late_names) + j}" for j in range(int(rng.integers(1, 4))))
+            names = [pick(late_names[-8:]) for _ in late]
+
+            def build(dd, r=r, late=late, names=names):
+                r = r.copy()
+                r["requestor_ip"][late] = [dd.intern_ip(x) for x in names]
+                return r
+            ev.append(("wait", st["now"], build))
+        else:
+            ev.append(("wait", st["now"], r))
+        st["waits"] += 1
+        st["issued"] += n
+        between()
+
+    def stretch_n() -> int:
+        lo, hi = _SIZE_CLASSES[size]
+        return int(rng.integers(max(lo, K + 2), hi + 1))  # (room for every digest of the stretch)
+
+    def facts(item: str) -> None:
+        """One heartbeat that changes a slot fact or a flag but keeps slot_b (else: a new scratch layout)."""
+        before = slot_b()
+        for _ in range(200):
+            p = pick(movers())
+            s = sv[p][1]
+            if item == "load":
+                t = replace(s, current_load=int(rng.integers(0, s.num_processors + 4)))
+            elif item == "nproc":
+                t = replace(s, num_processors=int(rng.choice([32, 64, 96, 128, s.num_processors + 1])))
+            elif item == "max-tasks-0":
+                t = replace(s, max_tasks=0)
+            elif item == "max-tasks-back":
+                back = [(q, m0) for loc, m0 in saved_mt for q, (_, x) in enumerate(sv) if x.observed_location == loc]
+                if back and rng.random() < 0.9:
+                    p, m0 = back[0]
+                    s = sv[p][1]
+                    t = replace(s, max_tasks=m0)
+                else:
+                    t = replace(s, max_tasks=s.num_processors * 40 // 100 if s.max_tasks == 0 else s.max_tasks + 1)
+            elif item == "low-memory":
+                t = replace(s, memory_available_in_bytes=40 * GiB if s.memory_available_in_bytes < 10 * GiB else 5 * GiB)
+            else:
+                t = replace(s, priority=_abi.PRIORITY_USER if s.priority == _abi.PRIORITY_DEDICATED else
+                            _abi.PRIORITY_DEDICATED)
+            if t == s:
+                continue
+            sv[p] = (sv[p][0], t)
+            if slot_b() == before:
+                sv[p] = (sv[p][0], s)
+                if item == "max-tasks-0":
+                    saved_mt.append((s.observed_location, s.max_tasks))
+                if item == "max-tasks-back":
+                    saved_mt[:] = [x for x in saved_mt if x[0] != s.observed_location]
+                hb(p, t)
+                return
+            sv[p] = (sv[p][0], s)
+        raise AssertionError(f"solo_stream({seed}): no {item} heartbeat keeps slot_b")
+
+    def perturb(item: str) -> None:
+        nonlocal classes, made
+        asked = [c for c in classes if c != zero]
+        if item == "version-drop-last":  # every eligible servant of one asked-for digest below its min_version
+            k = pick(asked or [zero])
+            dropped.append(k)
+            for p in holders(k):
+                s = sv[p][1]
+                if sv[p][0] not in pins and s.version >= mv[k]:
+                    hb(p, replace(s, version=int(rng.choice([mv[k] - 1, -1]))))
+        elif item == "version-up":  # those servants back up (else one servant)
+            ps = holders(dropped.pop()) if dropped else [pick(movers())]
+            for p in ps:
+                if sv[p][0] not in pins:
+                    hb(p, replace(sv[p][1], version=9))
+        elif item == "version-down":  # one servant below its digest's min_version
+            ps = [p for p in movers() if sv[p][1].version >= mv[digest_of(sv[p][1])]] or movers()
+            p = pick(ps)
+            hb(p, replace(sv[p][1], version=min(mv[digest_of(sv[p][1])], 9) - 1))
+        elif item in ("load", "nproc", "max-tasks-0", "max-tasks-back", "low-memory", "priority"):
+            facts(item)
+        elif item == "keepalive":
+            ev.append(("keepalive", st["now"], None, 15.0))
+        elif item == "free-unknown":  # ids never handed out, one of them twice
+            bogus = [st["issued"] + 10_000_000 + int(x) for x in rng.integers(0, 1000, 3)]
+            ev.append(("free", np.asarray(bogus + bogus[:1], dtype=np.uint64)))
+        elif item == "notify-bogus":
+            ev.append(("notify_own", pick(movers()), int(rng.integers(1 << 30)),
+                       [st["issued"] + 20_000_000, st["issued"] + 20_000_001]))
+        elif item == "tick-leases":
+            st["now"] += 0.02
+            ev.append(("tick", st["now"]))
+        elif item == "tiny":
+            batch(int(rng.integers(1, 9)))
+        elif item == "digest-set":  # the first holder of a digest, where it may move: the components are renumbered
+            firsts = [holders(k)[0] for k in range(K) if holders(k)]
+            ok = lambda p: sv[p][0] not in pins and len(holders(digest_of(sv[p][1]))) > 2  # noqa: E731
+            p = pick([p for p in firsts if ok(p)] or [p for p in movers() if ok(p)])
+            s = sv[p][1]
+            k = (digest_of(s) + 1 + int(rng.integers(0, K - 1))) % K
+            hb(p, replace(s, environments=[dgs[k]] * len(s.environments)))
+        elif item == "new-servant":
+            sv.append((made, new_servant(made, made % K)))
+            made += 1
+            ev.append(("hb", st["now"], sv[-1][1], 1e6))
+        elif item == "servant-expiry":
+            p = pick([p for p in movers() if len(holders(digest_of(sv[p][1]))) > 2])
+            ev.append(("hb", st["now"], sv[p][1], 0.001))
+            del sv[p]
+            st["now"] += 0.002
+            ev.append(("tick", st["now"]))
+        elif item == "new-min-version" and asked:  # from this batch on
+            k = pick(asked)
+            mv[k] = int(rng.choice([x for x in (0, 6, 7, 8, 9) if x != mv[k]]))
+            batch(stretch_n())
+        elif item in ("new-digest", "new-min-version"):  # a held digest the table lacks, from this batch on
+            missing = [k for k in range(K) if k not in classes and holders(k)]
+            if missing:
+                classes = sorted(classes + [missing[0]])
+            else:  # every held digest is asked for: a new min_version instead
+                k = pick(asked or [zero])
+                mv[k] = int(rng.choice([x for x in (0, 6, 7, 8, 9) if x != mv[k]]))
+            batch(stretch_n())
+        elif item == "self":
+            batch(stretch_n(), self_req=True)
+        elif item == "two-min-versions":
+            n = stretch_n()
+            k = np.asarray(classes)[rng.integers(0, len(classes), n)]
+            k[: len(classes)] = classes
+            m = np.asarray([mv[int(x)] for x in k], dtype=np.uint32)
+            two = pick(asked or [zero])
+            other = mv[two] - 1 if 0 < mv[two] <= 9 else 1
+            m[(k == two) & (rng.random(n) < 0.5)] = other
+            m[len(classes)] = other
+            k[len(classes)] = two
+            batch(n, k=k, m=m)
+        elif item == "size-class":
+            lo, hi = _SIZE_CLASSES[int(rng.choice([c for c in _SIZE_CLASSES if c != size]))]
+            batch(int(rng.integers(lo, hi + 1)))
+        elif item == "class-bound":  # every digest at enough min_versions for 40+ classes: the bound grows
+            per = -(-40 // K)  # (a "self" batch may have taken it from 16 to 32 already)
+            n = max(stretch_n(), K * per)
+            k = rng.integers(0, K, n)
+            m = rng.integers(0, per, n).astype(np.uint32)
+            k[: K * per] = np.repeat(np.arange(K), per)
+            m[: K * per] = np.tile(np.arange(per, dtype=np.uint32), K)
+            batch(n, k=k, m=m)
+        else:  # pragma: no cover
+            raise KeyError(item)
+
+    order = list(SOLO_MENU)
+    rng.shuffle(order)
+    target = 3 << 16 if wrap else 0  # requests offered: enough that the task ids handed out pass 2^17
+    passes = 0
+    while True:
+        passes += 1
+        for item in order:
+            if grow and st["issued"] >= 20_000 and "pin_from" not in st:
+                ev.append(("free_frac", int(rng.integers(1 << 30)), 1.0))  # the pinned window starts here
+                st["pin_from"], st["pinned"] = st["issued"], True
+            elif st["pinned"] and st["issued"] - st["pin_from"] >= 90_000:
+                st["pinned"] = False
+                ev.append(("free_frac", int(rng.integers(1 << 30)), 1.0))  # the pinned grants go
+            for _ in range(int(rng.integers(3, 5))):  # a steady stretch
+                batch(stretch_n())
+            if st["pinned"]:
+                ev.append(("keepalive", st["now"], None, 15.0))
+            at = st["waits"]
+            perturb(item)
+            checks.append((at if item in _SOLO_BATCHES else st["waits"], item, SOLO_MENU[item]))
+        if st["issued"] >= target and not st["pinned"]:
+            break
+        order = [x for x in SOLO_MENU if x != "class-bound"]  # (the bound has grown; it stays)
+        rng.shuffle(order)
+    for _ in range(3):
+        batch(stretch_n())
+    ev.append(("state",))
+    return Stream(f"solo-{seed}", ev, {"seed": seed, "servants": n_servants, "digests": K, "wrap": wrap, "grow": grow,
+                                       "checks": checks, "waits": st["waits"], "passes": passes})
 
 
 # ---------------------------------------------------------------------------

@@ -61,6 +61,8 @@ struct TopoView {  // the parts of the topology the class kernels need
   // null when some component holds more than 64 digests (the CSR above is walked instead)
   const unsigned long long* sv_emask;
   const uint32_t* env_local;
+  // per requestor IP (< n_ips): bit c = some servant of component c (< 64) is on that IP (ip_off / ip_sv in one load)
+  const unsigned long long* ip_comp_mask;
 };
 
 __device__ __forceinline__ uint32_t cls_hash(unsigned long long key) {
@@ -134,24 +136,36 @@ __device__ __forceinline__ void cls_insert_one(uint32_t env, uint32_t mv, uint32
   }
 }
 
-// A request's class in the table a previous solo solve kept (fused.cuh, speculative variant), or kNone for an unknown
-// digest or one no component holds (EnvironmentNotFound, as cls_insert_one skips them).  `miss`: the kept table cannot
-// decide the request -- its class is not in the table, or the requestor's IP is that of a servant of the component
-// (which would take it off the data-parallel path).
+// The kept class table as seen from a digest (fused.cuh, speculative variant): kept_env[env] = {class, its min_version,
+// its component, 0}, where the class is the one the digest's component holds in the table -- a kept table holds at most
+// one class per component, and only if that class is of this digest -- or x = kNone (no component holds the digest) or
+// x = kKeptNoClass (its component holds no class of this digest).
+constexpr uint32_t kKeptNoClass = 0xFFFFFFFEu;
+
+// A request's class in the table a previous solo solve kept, or kNone for an unknown digest or one no component holds
+// (EnvironmentNotFound, as cls_insert_one skips them).  `miss`: the kept table cannot decide the request -- its class is
+// not in the table, or the requestor's IP is that of a servant of the component (which would take it off the
+// data-parallel path).  Two independent loads after the request: the digest's kept_env word and the IP's component mask
+// (the IP CSR is walked only for a component beyond the mask's 64 bits).
 __device__ __forceinline__ uint32_t kept_class(uint32_t env, uint32_t mv, uint32_t ip, const TopoView& t,
-                                               const ClassTable& ct, bool& miss) {
+                                               const uint4* __restrict__ kept_env, bool& miss) {
   if (env >= t.n_envs) return kNone;
-  const uint32_t comp = t.env_comp[env];
-  if (comp == kNone) return kNone;
-  const uint32_t slot = cls_find(ct.keys, ((unsigned long long)env << 32) | mv);
-  const uint32_t cls = slot != kNone ? ct.slot_cls[slot] : kNone;
-  if (cls == kNone) miss = true;
-  if (ip < t.n_ips) {
+  const uint4 w = kept_env[env];
+  const unsigned long long ipm = ip < t.n_ips ? t.ip_comp_mask[ip] : 0ull;
+  if (w.x == kNone) return kNone;
+  if (w.x == kKeptNoClass || w.y != mv) {
+    miss = true;
+    return kNone;
+  }
+  const uint32_t comp = w.z;
+  if (comp < 64) {
+    if ((ipm >> comp) & 1ull) miss = true;
+  } else if (ip < t.n_ips) {
     for (uint32_t u = t.ip_off[ip], e = t.ip_off[ip + 1]; u < e; ++u) {
       if (t.sv_comp[t.ip_sv[u]] == comp) miss = true;
     }
   }
-  return cls;
+  return w.x;
 }
 
 __global__ void __launch_bounds__(256) k_cls_insert(const yd_task_req* __restrict__ reqs,
@@ -419,10 +433,14 @@ __global__ void __launch_bounds__(256) k_slot_records(const unsigned long long* 
 // barriers per chunk, whatever the number of classes.
 constexpr uint32_t kListChunk = 64;
 
+// The ballots of one chunk of lists, staged for the counts (list_count_tile, list_count_tile_kept: one array per
+// kernel, whichever of the two it calls).
+__shared__ uint32_t s_count_bal[kListChunk][32];
+
 __device__ __forceinline__ void list_count_tile(uint32_t tile, uint32_t m, const SlotDecode& d, const TopoView& t,
                                                 const ClassTable& ct, const ServantArrays& sv, uint32_t n_tiles,
                                                 uint32_t* __restrict__ counts, uint32_t* __restrict__ balg) {
-  __shared__ uint32_t bal[kListChunk][32];
+  auto& bal = s_count_bal;
   const uint32_t ncls = min(ct.meta[0], ct.cls_bound);
   const uint32_t nmerge = min(ct.meta[2], ct.cls_bound - ncls);
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -446,6 +464,52 @@ __device__ __forceinline__ void list_count_tile(uint32_t tile, uint32_t m, const
       if (lane == 0) { bal[c - c0][warp] = b; my_row[c * 32 + warp] = b; }
     }
     __syncthreads();
+    for (uint32_t c = c0 + warp; c < c1; c += 32) {
+      const uint32_t cnt = __reduce_add_sync(0xffffffffu, (uint32_t)__popc(bal[c - c0][lane]));
+      if (lane == 0) counts[c * n_tiles + tile] = cnt;
+    }
+    __syncthreads();  // the ballots have been consumed
+  }
+}
+
+// list_count_tile against a kept class table (fused.cuh, speculative variant; ncls classes, no merge pseudo-classes: a
+// kept table comes from a solo solve): the same ballot words and counts, with a third of the work.  A slot tile is bound
+// by its gathers from random servants and by one eligibility test per (slot, class), not by its load latency; but a kept
+// table holds at most one class per component, so a slot is in one list at most -- that of kept_sv[servant] (the class
+// of its component, if it holds the class's digest; written with the table), if the servant's version is high enough.
+// So: three gathers per slot (run, kept_sv, version) instead of four to five, one test, and the lanes of a warp grouped
+// by list (__match_any_sync) instead of one ballot per class.  s_mv: the classes' min_versions in shared memory, loaded
+// by the block's first call (`facts`).
+__device__ __forceinline__ void list_count_tile_kept(uint32_t tile, uint32_t m, uint32_t ncls, const SlotDecode& d,
+                                                     const ClassTable& ct, const ServantArrays& sv,
+                                                     const uint32_t* __restrict__ kept_sv, uint32_t n_tiles,
+                                                     uint32_t* __restrict__ counts, uint32_t* __restrict__ balg,
+                                                     uint32_t* s_mv, bool& facts) {
+  auto& bal = s_count_bal;
+  uint32_t* const bal_flat = &bal[0][0];
+  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const uint32_t i = tile * kListTile + tid;
+  const uint2 rec = i < m ? d.rec[i] : make_uint2(kNone, 0u);
+  const bool load_facts = !facts && tid < ncls;
+  const uint32_t f_mv = load_facts ? ct.cls_mv[tid] : 0u;
+  const uint32_t pos = rec.x != kNone ? rec.x : 0u;  // (a dead slot reads servant 0's facts: no branch before the loads)
+  const uint32_t run = d.run[pos], ver = (uint32_t)sv.version[pos];
+  uint32_t cls = kept_sv[pos];
+  if (load_facts) s_mv[tid] = f_mv;
+  if (!facts) __syncthreads();
+  facts = true;
+  // a slot outside its row, one the servant has filled already, or a servant below the class's min_version: no list
+  if (rec.x == kNone || rec.y < run || cls >= ncls || ver < s_mv[cls]) cls = kNone;
+  uint32_t* my_row = balg + size_t(tile) * ct.cls_bound * 32;
+  for (uint32_t c0 = 0; c0 < ncls; c0 += kListChunk) {
+    const uint32_t c1 = min(c0 + kListChunk, ncls);
+    for (uint32_t k = tid; k < (c1 - c0) * 32; k += kListTile) bal_flat[k] = 0;
+    __syncthreads();
+    const uint32_t key = (cls >= c0 && cls < c1) ? cls : kNone;
+    const uint32_t peers = __match_any_sync(0xffffffffu, key);  // = the ballot of list `key` in this warp
+    if (key != kNone && lane == (uint32_t)(__ffs(peers) - 1)) bal[key - c0][warp] = peers;
+    __syncthreads();
+    for (uint32_t k = tid; k < (c1 - c0) * 32; k += kListTile) my_row[c0 * 32 + k] = bal_flat[k];
     for (uint32_t c = c0 + warp; c < c1; c += 32) {
       const uint32_t cnt = __reduce_add_sync(0xffffffffu, (uint32_t)__popc(bal[c - c0][lane]));
       if (lane == 0) counts[c * n_tiles + tile] = cnt;

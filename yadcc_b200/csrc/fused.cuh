@@ -22,11 +22,14 @@
 //
 // E1 only numbers the classes, and a scheduler's class set -- (digest, min_version) pairs -- rarely changes from one
 // batch to the next.  So a solo solve whose class set is the one of the previous solo solve KEEPS its class table (keys,
-// slot_cls, cls_env / mv / comp, meta, comp_mode), and the next solo solve runs SPECULATIVELY on it, with one barrier:
+// slot_cls, cls_env / mv / comp, meta, comp_mode) and writes it out per digest and per servant (kept_env, kept_sv), and
+// the next solo solve runs SPECULATIVELY on it, with one barrier:
 //
-//   A   every request looked up in the kept table (kept_class) and ranked in its tile (rank_in_tile): its class and rank
-//       stay in registers, as tile t is handled by block t % G in both phases; list ballots and counts; eligible
-//       servants per class (servant versions and max_tasks change without a new topology)
+//   A   every request looked up in the kept table (kept_class: the digest's kept_env word and the IP's component mask,
+//       two independent loads) and ranked in its tile (rank_in_tile): its class and rank stay in registers, as tile t is
+//       handled by block t % G in both phases; list ballots and counts, one list per slot at most
+//       (list_count_tile_kept); eligible servants per class (servant versions and max_tasks change without a new
+//       topology)
 //   --  barrier
 //   B   P6 as above (the lite selection, closed-form task ids).  The last block resets the barrier words, nothing else.
 //
@@ -125,8 +128,19 @@ struct FusedArgs {
   uint32_t loff_cache_words;  // dynamic shared memory of the launch, in words
   uint32_t lite;              // solo: no leader scans -- every block derives the offsets it needs from the raw counts
   uint32_t spec;              // solo, speculative: the class table kept from the last solo solve, one grid barrier
-  unsigned long long* prof;  // debug (YDSCHED_FUSED_PROF): block 0 stamps %globaltimer at every phase boundary, else null
+  uint4* kept_env;            // [n_envs] the kept class table per digest (classes.cuh: kept_class) ...
+  uint32_t* kept_sv;          // [n_servants] ... and per servant (list_count_tile_kept); both written with the table
+  unsigned long long* prof;  // debug (YDSCHED_FUSED_PROF): %globaltimer stamps (kProfHead / kProfBlockWords), else null
 };
+
+// YDSCHED_FUSED_PROF: block 0 stamps every phase boundary into prof[0 .. 9).  The speculative variant also stamps, per
+// block b, prof[kProfHead + b * kProfBlockWords + k]: k = 0 start, 1..3 end of its first three items of phase A, 4
+// barrier arrival, 5 departure, 6 end of phase B; word 7 = the kinds of those items (4 bits each, FusedItem) | the
+// number of items << 16.
+constexpr uint32_t kProfHead = 16;
+constexpr uint32_t kProfBlockWords = 8;
+constexpr uint32_t kProfMaxItems = 3;
+enum FusedItem : uint32_t { kItemRequests = 1, kItemSlots = 2, kItemClass = 3 };
 
 __device__ __forceinline__ unsigned long long fused_now() {
   unsigned long long t;
@@ -135,6 +149,9 @@ __device__ __forceinline__ unsigned long long fused_now() {
 }
 __device__ __forceinline__ void fused_stamp(const FusedArgs& a, int k) {
   if (a.prof && blockIdx.x == 0 && threadIdx.x == 0) a.prof[k] = fused_now();
+}
+__device__ __forceinline__ void fused_bstamp(const FusedArgs& a, uint32_t k, unsigned long long v) {
+  if (a.prof && threadIdx.x == 0) a.prof[kProfHead + blockIdx.x * kProfBlockWords + k] = v;
 }
 
 // Pull a table into L2 while the first phase streams the requests: the bench flushes L2 between solves and a scheduler
@@ -240,6 +257,29 @@ __device__ __forceinline__ unsigned long long fused_classes_fp(const unsigned lo
   cnt = fused_block_sum(cnt);
   mix = fused_block_sum(mix);
   return ((unsigned long long)(cnt + 1) << 32) | mix;
+}
+
+// The kept table per digest (kept_env, classes.cuh) and per servant (kept_sv: the class of its component if it holds
+// that class's digest, else kNone), by the one block that keeps the table.  First every digest of a component says "no
+// class" and every servant kNone, then each class writes its digest and walks its component's servants.  (Each component
+// of a kept table holds one class at most, so nothing is written twice.)
+__device__ __forceinline__ void fused_keep_env(const FusedArgs& a) {
+  const uint32_t ncls = min(a.ct.meta[0], a.ct.cls_bound);
+  for (uint32_t e = threadIdx.x; e < a.t.n_envs; e += 1024) {
+    a.kept_env[e] = make_uint4(a.t.env_comp[e] == kNone ? kNone : kKeptNoClass, 0u, 0u, 0u);
+  }
+  for (uint32_t p = threadIdx.x; p < a.n_servants; p += 1024) a.kept_sv[p] = kNone;
+  __syncthreads();
+  for (uint32_t c = threadIdx.x; c < ncls; c += 1024) {
+    a.kept_env[a.ct.cls_env[c]] = make_uint4(c, a.ct.cls_mv[c], a.ct.cls_comp[c], 0u);
+  }
+  for (uint32_t c = 0; c < ncls; ++c) {
+    const uint32_t comp = a.ct.cls_comp[c], env = a.ct.cls_env[c];
+    for (uint32_t i = a.t.comp_sv_off[comp] + threadIdx.x, e = a.t.comp_sv_off[comp + 1]; i < e; i += 1024) {
+      const uint32_t pos = a.t.comp_sv[i];
+      if (servant_has_env(a.t, pos, env)) a.kept_sv[pos] = c;
+    }
+  }
 }
 
 // In-place exclusive scan of data[0 .. cells) by one block of 1024 threads (8 values per thread and round).
@@ -417,6 +457,14 @@ __global__ void __launch_bounds__(1024, 1) k_fused_front(FusedArgs a) {
   __shared__ DynParams s_dyn;
   __shared__ unsigned long long s_seq, s_zc_in, s_zc_out, s_kept_fp;
   const uint32_t tid = threadIdx.x, G = gridDim.x;
+  if (a.prof && tid == 0) {
+    const unsigned long long t0 = fused_now();
+    if (blockIdx.x == 0) a.prof[0] = t0;
+    if (a.spec) {
+      fused_bstamp(a, 0, t0);
+      fused_bstamp(a, 7, 0);
+    }
+  }
   if (tid == 0) {
     const FusedScalars sc = a.sc_dev ? *a.sc_dev : a.sc;
     s_dyn = sc.dyn;
@@ -433,12 +481,14 @@ __global__ void __launch_bounds__(1024, 1) k_fused_front(FusedArgs a) {
   const uint32_t lt_live = min((m + kListTile - 1) / kListTile, a.n_ltiles);  // slot tiles that hold slots
   const ReqView rv{a.reqs, a.reqs16};
 
-  fused_stamp(a, 0);
   if (tid < 64) s_seen[tid] = kClsEmpty;
   __syncthreads();
   {
     const size_t S4 = size_t(a.n_servants) * 4;
-    if (a.spec) fused_prefetch(a.ct.keys, kClsTableSize * 8);
+    if (a.spec) {
+      fused_prefetch(a.kept_env, size_t(a.t.n_envs) * sizeof(uint4));
+      fused_prefetch(a.t.ip_comp_mask, size_t(a.t.n_ips) * 8);
+    }
     fused_prefetch(a.dec.rec, size_t(m) * 8);
     fused_prefetch(a.sv.run, S4);
     fused_prefetch(a.sv.version, S4);
@@ -458,24 +508,37 @@ __global__ void __launch_bounds__(1024, 1) k_fused_front(FusedArgs a) {
     // ---- A: requests against the kept class table, list ballots and counts, eligible servants per class ------------
     // Request tiles are the first items, so tile t is handled by block t % G here and in B below: the class and rank of
     // a request stay in this thread's registers.
+    __shared__ uint32_t s_cls_mv[kMaxClasses];
     ncls = min(a.ct.meta[0], a.ct.cls_bound);
     nlists = min(a.ct.meta[3], a.ct.cls_bound);
-    bool miss = false;
+    bool miss = false, facts = false;
     const uint32_t items = nb_live + lt_live + ncls;
+    uint32_t kinds = 0;  // (YDSCHED_FUSED_PROF)
     for (uint32_t it = blockIdx.x, k = 0; it < items; it += G, ++k) {
+      uint32_t kind;
       if (it < nb_live) {
         uint32_t env, mv, ip, cls = kNone;
-        if (fused_fetch_req(a, rv, zc_in, it, n, env, mv, ip)) cls = kept_class(env, mv, ip, a.t, a.ct, miss);
+        if (fused_fetch_req(a, rv, zc_in, it, n, env, mv, ip)) cls = kept_class(env, mv, ip, a.t, a.kept_env, miss);
         const uint32_t rank = rank_in_tile(it, cls, a.ct, a.n_rtiles, a.rank_cnt);
         const uint32_t cr = (rank << 16) | (cls & 0xffffu);
         if (k == 0) spec_cr0 = cr;
         else if (k == 1) spec_cr1 = cr;
         else miss = true;  // (more request tiles than two per block: the host does not speculate on such batches)
+        kind = kItemRequests;
       } else if (it < nb_live + lt_live) {
-        list_count_tile(it - nb_live, m, a.dec, a.t, a.ct, a.sv, a.n_ltiles, a.list_cnt, a.list_bal);
+        list_count_tile_kept(it - nb_live, m, ncls, a.dec, a.ct, a.sv, a.kept_sv, a.n_ltiles, a.list_cnt, a.list_bal,
+                             s_cls_mv, facts);
+        kind = kItemSlots;
       } else {
         cls_elig_class(it - nb_live - lt_live, a.t, a.ct, a.sv);
+        kind = kItemClass;
       }
+      if (a.prof && k < kProfMaxItems) {
+        __syncthreads();  // (the item's end: all of its threads are done)
+        fused_bstamp(a, 1 + k, fused_now());
+        kinds |= kind << (4 * k);
+      }
+      if (a.prof) fused_bstamp(a, 7, kinds | (min(k + 1, 0xffffu) << 16));
     }
     // slot tiles beyond the table's end hold no members (the lists' row scans below read them; nothing re-zeroes them)
     const uint32_t tail = a.n_ltiles - lt_live;
@@ -483,8 +546,10 @@ __global__ void __launch_bounds__(1024, 1) k_fused_front(FusedArgs a) {
     if (__syncthreads_or(miss) && tid == 0) atomicExch(&a.ct.meta[1], kFlagSpecMiss);
     lite = true;  // (the host speculates only when the lists' offsets fit in shared memory)
     fused_stamp(a, 1);
+    fused_bstamp(a, 4, fused_now());
     fused_barrier(a.bar, 1);
     fused_stamp(a, 2);
+    fused_bstamp(a, 5, fused_now());
     if (*reinterpret_cast<volatile uint32_t*>(&a.ct.meta[1]) != 0) {
       // nothing is decided: the last block reports and leaves the scratch clean (the kept table too) for the replay
       if (fused_done_last(a.bar)) {
@@ -651,6 +716,10 @@ __global__ void __launch_bounds__(1024, 1) k_fused_front(FusedArgs a) {
     }
   }
   fused_stamp(a, 7);
+  if (a.spec && a.prof) {
+    __syncthreads();  // (every thread of the block is done with B)
+    fused_bstamp(a, 6, fused_now());
+  }
   // ---- solo: the block that finishes last reports to the host and leaves the scratch as the next solve expects it ----
   // A speculative solve resets the barrier words alone: the class table stays, and everything else it wrote is
   // rewritten by the next one before it is read.  Any other solo solve keeps its class table when its class set is the
@@ -664,8 +733,12 @@ __global__ void __launch_bounds__(1024, 1) k_fused_front(FusedArgs a) {
       fused_report(a, s_seq, a.counters->granted, fp);
       __syncthreads();  // (the report reads meta[], which lies in the region zeroed below)
       uint32_t from = 0;
-      if (fp == s_kept_fp) from = kKeptClsWords / 4;
-      else for (uint32_t i = tid; i < kClsTableSize; i += 1024) a.clean_keys[i] = kClsEmpty;
+      if (fp == s_kept_fp) {
+        from = kKeptClsWords / 4;
+        fused_keep_env(a);
+      } else {
+        for (uint32_t i = tid; i < kClsTableSize; i += 1024) a.clean_keys[i] = kClsEmpty;
+      }
       for (uint32_t i = from + tid; i < a.clean_zero_vec; i += 1024) a.clean_zero[i] = make_uint4(0u, 0u, 0u, 0u);
     }
     if (a.prof && tid == 0) a.prof[8] = fused_now();

@@ -166,7 +166,8 @@ struct yd_sched {
 
   // topology on device
   DevBuf d_env_comp, d_env_local, d_comp_sv_off, d_comp_sv, d_comp_mask_off, d_comp_nwarps, d_envmask,
-      d_sv_comp, d_sv_local, d_ip_off, d_ip_sv;
+      d_sv_comp, d_sv_local, d_ip_off, d_ip_sv, d_ip_comp_mask;
+  DevBuf d_kept_env, d_kept_sv;  // the kept class table per digest / per servant (fused.cuh)
   uint32_t n_comps = 0, n_envs_dev = 0, n_ips_dev = 0, max_warps = 1, max_comp_servants = 0;
   bool wide = false;
   PinBuf h_topo;
@@ -479,6 +480,11 @@ void yd_sched::SyncTopology() {
     ip_sv.insert(ip_sv.end(), by_ip[k].begin(), by_ip[k].end());
   }
   ip_off[NI] = (uint32_t)ip_sv.size();
+  // the same per IP as one word: the components (< 64) with a servant on it (the speculative solve's self-request test)
+  std::vector<unsigned long long> ip_comp_mask(std::max(NI, 1u), 0ull);
+  for (uint32_t k = 0; k != NI; ++k) {
+    for (uint32_t i : by_ip[k]) if (sv_comp[i] < 64) ip_comp_mask[k] |= 1ull << sv_comp[i];
+  }
 
   auto up = [&](DevBuf& b, const void* src, size_t bytes) {
     b.ensure(std::max<size_t>(bytes, 4));
@@ -495,6 +501,9 @@ void yd_sched::SyncTopology() {
   up(d_sv_local, sv_local.data(), size_t(S) * 4);
   up(d_ip_off, ip_off.data(), size_t(NI + 1) * 4);
   up(d_ip_sv, ip_sv.data(), ip_sv.size() * 4);
+  up(d_ip_comp_mask, ip_comp_mask.data(), ip_comp_mask.size() * 8);
+  d_kept_env.ensure(std::max<size_t>(size_t(E) * 16, 16));  // (both written by the solve that keeps a class table)
+  d_kept_sv.ensure(std::max<size_t>(size_t(S) * 4, 4));
   // digest ids per servant (CSR) for class-eligibility tests on the device
   std::vector<uint32_t> env_off(S + 1, 0), env_flat;
   for (uint32_t i = 0; i != S; ++i) {
@@ -599,14 +608,17 @@ yd_sched* yd_create(const yd_config* cfg) {
   s->host_prof = getenv("YDSCHED_HOST_PROF") != nullptr;
   s->d_report.ensure(sizeof(yd::FusedHostIO));
   s->fused_prof = getenv("YDSCHED_FUSED_PROF") != nullptr;
-  s->d_fused_prof.ensure(128);
-  YD_CUDA_CHECK(cudaMemset(s->d_fused_prof.p, 0, 128));
   {
     int sms = 0, per_sm = 0;
     YD_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, cfg->device));
     YD_CUDA_CHECK(cudaFuncSetAttribute(yd::k_fused_front, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
     YD_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, yd::k_fused_front, 1024, 64 * 1024));
     s->fused_grid = per_sm >= 1 ? (uint32_t)sms : 0u;  // (0: the kernel does not fit an SM -- never on sm_90a; the pipeline is used)
+  }
+  {
+    const size_t prof_bytes = (yd::kProfHead + size_t(s->fused_grid) * yd::kProfBlockWords) * 8;
+    s->d_fused_prof.ensure(prof_bytes);
+    YD_CUDA_CHECK(cudaMemset(s->d_fused_prof.p, 0, prof_bytes));
   }
   s->dump_env = getenv("YDSCHED_DUMP") != nullptr;
   s->debug_env = getenv("YDSCHED_DEBUG") != nullptr;
@@ -644,7 +656,8 @@ void yd_destroy(yd_sched* s) {
   for (DevBuf* b : {&s->d_nproc, &s->d_load, &s->d_maxt, &s->d_flags, &s->d_ver, &s->d_run, &s->d_ever,
                     &s->d_run_tmp, &s->d_ever_tmp, &s->d_remap, &s->d_env_comp, &s->d_env_local,
                     &s->d_comp_sv_off, &s->d_comp_sv, &s->d_comp_mask_off, &s->d_comp_nwarps, &s->d_envmask,
-                    &s->d_sv_comp, &s->d_sv_local, &s->d_ip_off, &s->d_ip_sv, &s->d_t_exp, &s->d_t_srv,
+                    &s->d_sv_comp, &s->d_sv_local, &s->d_ip_off, &s->d_ip_sv, &s->d_ip_comp_mask, &s->d_kept_env, &s->d_kept_sv,
+                    &s->d_t_exp, &s->d_t_srv,
                     &s->d_t_flags, &s->d_reqs, &s->d_res, &s->d_out, &s->d_blk, &s->d_row_off, &s->d_row_len,
                     &s->d_codes, &s->d_ids, &s->d_ok, &s->d_counters, &s->d_sv_env_off, &s->d_sv_envs,
                     &s->d_comp_mode, &s->d_sv_emask, &s->d_slot_rec, &s->d_slot_owner, &s->d_sort_k[0], &s->d_sort_k[1], &s->d_sort_v[0],
@@ -737,6 +750,7 @@ yd::TopoView MakeTopo(yd_sched* s) {
   t.comp_sv = s->d_comp_sv.as<uint32_t>();
   t.sv_emask = s->emask_ok ? s->d_sv_emask.as<unsigned long long>() : nullptr;
   t.env_local = s->d_env_local.as<uint32_t>();
+  t.ip_comp_mask = s->d_ip_comp_mask.as<unsigned long long>();
   return t;
 }
 
@@ -1161,6 +1175,8 @@ uint32_t LaunchFused(yd_sched* s, uint32_t N, size_t slot_b, bool capturing, boo
   a.loff_cache_words = (uint32_t)(dyn / 4);
   a.lite = s->fused_lite ? 1u : 0u;
   a.spec = spec ? 1u : 0u;
+  a.kept_env = s->d_kept_env.as<uint4>();
+  a.kept_sv = s->d_kept_sv.as<uint32_t>();
   yd::k_fused_front<<<grid, 1024, dyn, st>>>(a);
   s->last_fused = a;
   s->last_fused_grid = grid;
@@ -1645,6 +1661,14 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
         fprintf(stderr, "ydsched: fused variant 4 (speculative) n %u ns: A %llu barrier %llu B %llu total %llu (+tail %lld)\n", N,
                 t[1] - t[0], t[2] - t[1], t[7] - t[2], t[7] - t[0], (long long)(t[8] - t[7]));
       }
+      // every block's stamps (fused.cuh: kProfBlockWords), for tools/dev/phase_prof.py
+      const uint32_t G = s->last_fused_grid;
+      std::vector<unsigned long long> b(size_t(G) * yd::kProfBlockWords);
+      YD_CUDA_CHECK(cudaMemcpy(b.data(), s->d_fused_prof.as<unsigned long long>() + yd::kProfHead, b.size() * 8,
+                               cudaMemcpyDeviceToHost));
+      std::string line = "ydsched: fused blocks " + std::to_string(G) + " last_end " + std::to_string(t[8]) + " stamps";
+      for (unsigned long long v : b) line += " " + std::to_string(v);
+      fprintf(stderr, "%s\n", line.c_str());
     } else if (s->fused_prof && variant) {
       unsigned long long t[9];
       YD_CUDA_CHECK(cudaMemcpy(t, s->d_fused_prof.p, sizeof t, cudaMemcpyDeviceToHost));

@@ -270,8 +270,13 @@ void yd_wait_for_starting_new_tasks_packed(yd_sched* s, int64_t now_ns, const yd
  * window of time can stage them as they arrive and start the solve when the batch closes:
  * yd_stage_requests copies reqs[0..n) into the handle's device-side queue (synchronously: the
  * array may be reused at once); yd_wait_for_staged_tasks decides the first n staged requests
- * exactly like yd_wait_for_starting_new_tasks would.  Staged requests stay valid until the
- * next yd_stage_requests / yd_wait_for_starting_new_tasks(reqs != NULL) call. */
+ * exactly like yd_wait_for_starting_new_tasks would.  Staged requests stay valid, and may be
+ * decided again, until the next call that replaces or drops them:
+ *  - yd_stage_requests replaces them;
+ *  - yd_wait_for_starting_new_tasks and yd_wait_for_starting_new_tasks_packed with n > 0 drop them
+ *    (the batch goes through the same device-side queue);
+ *  - yd_filter_and_wait_for_starting_new_tasks with n > 0 replaces them with the requests it
+ *    offered, in order (none if every request was filtered out). */
 void yd_stage_requests(yd_sched* s, const yd_task_req* reqs, size_t n);
 void yd_wait_for_staged_tasks(yd_sched* s, int64_t now_ns, size_t n, yd_grant* out);
 /* n TaskDispatcher::KeepTaskAlive calls (cc:142-165); ok_out[i] is the bool. */
@@ -403,7 +408,9 @@ typedef struct yd_prefilter {
 /* verdict_out[i] (n bytes) = YD_FILTER_*; hits_out (n entries, may be NULL) = what
  * yd_running_index_find reports for request i; grants_out (capacity n): the decisions for the
  * OFFERED requests, in order.  Returns how many requests were offered.  Defined as the three calls
- * above applied in that order; the CUDA backend keeps the queue in HBM between the stages. */
+ * above applied in that order, the third as yd_stage_requests(offered) + yd_wait_for_staged_tasks:
+ * the offered requests stay staged afterwards.  The CUDA backend keeps the queue in HBM between the
+ * stages. */
 size_t yd_filter_and_wait_for_starting_new_tasks(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, size_t n,
                                                  const yd_prefilter* filter, uint8_t* verdict_out,
                                                  yd_running_hit* hits_out, yd_grant* grants_out);

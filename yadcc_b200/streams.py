@@ -26,6 +26,10 @@ Event kinds (tuples, first element is the kind):
                                               some bogus ids)
   ("running",)                                GetRunningTasks
   ("state",)                                  per-servant bookkeeping snapshot
+  ("filter", now, REQ array, cache_keys, task_digests)
+                                              one yd_filter_and_wait_for_starting_new_tasks call (keys: strings or
+                                              uint8 matrices, or None to skip that stage); traces the verdicts, the
+                                              in-flight hits and the grants of the offered requests
 
 Task ids are the ordinal of the grant (the reference starts at 0 and increments
 per grant, task_dispatcher.h:218, .cc:127), so "free"/"keepalive" events can
@@ -69,36 +73,85 @@ class Replayer:
     """Drives a TaskDispatcher with a Stream and records everything it returns."""
 
     def __init__(self, dispatcher: TaskDispatcher, *, pinned: bool = False, on_solve: Callable | None = None,
-                 batch_heartbeats: bool = False, packed: bool = False):
+                 batch_heartbeats: bool = False, packed: bool = False, staged: bool = False, seed: int = 0):
         """`batch_heartbeats`: runs of consecutive "hb" events with one timestamp go through
         keep_servants_alive, runs of consecutive "notify"/"notify_own" events through
-        notify_servants_running_tasks (one call each); the trace is the same by definition."""
+        notify_servants_running_tasks (one call each); the trace is the same by definition.
+
+        `staged`: solves go through the device-side queue (yd_stage_requests + yd_wait_for_staged_tasks).  The trace is
+        the same by definition.  Per solve, a generator seeded with `seed` picks how (`modes` records it):
+          "exact"   stage the batch, decide it;
+          "longer"  stage the batch followed by unrelated requests, decide the batch's prefix;
+          "host"    the plain (or packed) call with the batch in a host array, which drops the staged queue (see
+                    `_host_array` for how long the array lives);
+          "reuse"   (not picked: taken whenever the batch is a prefix of what is still staged, e.g. the requests a
+                    filtered call offered) decide it without staging again.
+        Staged grants land in one grant array reused across calls."""
         self.d = dispatcher
         self.batch_heartbeats = batch_heartbeats
         self.packed = packed  # solves go through yd_wait_for_starting_new_tasks_packed (16-byte requests, 8-byte grants)
         self.pinned = pinned
         self.on_solve = on_solve
+        self.staged = staged
+        self.rng = np.random.default_rng(seed)
+        self.modes: list[str] = []  # per solve call (staged mode), and "filter" per filtered call
+        self.staged_q: np.ndarray | None = None  # host copy of the handle's staged queue, None once dropped
+        self._host_bufs: list[np.ndarray] = []  # the host calls' request arrays, kept alive (see above)
+        self._gout = np.zeros(0, dtype=GRANT_DTYPE)
         self.pending = np.zeros(0, dtype=REQ_DTYPE)
         self.outstanding: dict[int, int] = {}  # task id -> servant index at grant time
         self.decisions = 0
         self.granted = 0
         self.solve_calls = 0
 
+    def _host_array(self, alloc: Callable, n: int) -> np.ndarray:
+        """A page-locked request array for one host call.  Staged mode keeps every one alive until the replay ends and
+        makes it at least 64 k requests long, so that a staged solve that read one of them instead of the device-side
+        queue would read other requests, inside a live allocation."""
+        if not self.staged:
+            return alloc(n)
+        self._host_bufs.append(alloc(max(n, 1 << 16)))
+        return self._host_bufs[-1][:n]
+
+    def _staged_mode(self, reqs: np.ndarray) -> str:
+        n, q = len(reqs), self.staged_q
+        if n and q is not None and len(q) >= n and (q[:n] == reqs).all():
+            return "reuse"
+        u = self.rng.random()
+        return "host" if u < 0.2 else "longer" if u < 0.6 else "exact"
+
     def _wait(self, now: float, reqs: np.ndarray) -> np.ndarray:
-        if self.packed:
+        mode = self._staged_mode(reqs) if self.staged else "host"
+        if self.staged:
+            self.modes.append(mode)
+        if mode != "host":
+            n = len(reqs)
+            if mode != "reuse":
+                q = np.ascontiguousarray(reqs)
+                if mode == "longer":  # unrelated requests behind the batch: the batch's own, rotated and reversed
+                    tail = np.roll(q, int(self.rng.integers(1, max(n, 2))))[::-1][: int(self.rng.integers(1, max(n, 1) + 1))]
+                    q = np.concatenate([q, tail])
+                self.d.stage_requests(q)
+                self.staged_q = q.copy()
+            if len(self._gout) < n:
+                self._gout = self.d.alloc_grants(2 * n) if self.pinned else np.zeros(2 * n, dtype=GRANT_DTYPE)
+            g = self.d.wait_for_staged_tasks(n, now, out=self._gout).copy()
+        elif self.packed:
             from .dispatcher import pack_requests
             if self.pinned:
-                buf = pack_requests(reqs, self.d.alloc_requests16(len(reqs)))
+                buf = pack_requests(reqs, self._host_array(self.d.alloc_requests16, len(reqs)))
                 g = self.d.wait_for_starting_new_tasks_packed(buf, now, out8=self.d.alloc_grants8(len(reqs)))
             else:
                 g = self.d.wait_for_starting_new_tasks_packed(pack_requests(reqs), now)
         elif self.pinned:
-            buf = self.d.alloc_requests(len(reqs))
+            buf = self._host_array(self.d.alloc_requests, len(reqs))
             buf[...] = reqs
             out = self.d.alloc_grants(len(reqs))
             g = self.d.wait_for_starting_new_tasks(buf, now, out=out).copy()
         else:
             g = self.d.wait_for_starting_new_tasks(np.ascontiguousarray(reqs), now).copy()
+        if mode == "host" and len(reqs):
+            self.staged_q = None
         self.decisions += len(reqs)
         ok = g["status"] == STATUS_GRANTED
         self.granted += int(ok.sum())
@@ -108,6 +161,23 @@ class Replayer:
         if self.on_solve:
             self.on_solve(self.d, reqs, g)
         return g
+
+    def _filter(self, now: float, reqs: np.ndarray, cache_keys, task_digests) -> list[np.ndarray]:
+        """One filtered call: [verdicts, in-flight hits, grants of the offered requests]."""
+        reqs = np.ascontiguousarray(reqs)
+        v, hits, g = self.d.filter_and_wait_for_starting_new_tasks(reqs, cache_keys, task_digests, now)
+        g = g.copy()
+        if len(reqs):  # the offered requests are the staged queue now (ydsched.h)
+            self.staged_q = reqs[v == 0].copy()
+        self.modes.append("filter")
+        self.decisions += len(g)
+        ok = g["status"] == STATUS_GRANTED
+        self.granted += int(ok.sum())
+        for tid, sidx in zip(g["task_id"][ok].tolist(), g["servant_index"][ok].tolist()):
+            self.outstanding[tid] = sidx
+        if self.on_solve:
+            self.on_solve(self.d, reqs[v == 0], g)
+        return [v.copy(), hits.copy(), g]
 
     def _notify_args(self, ev):
         """(location, tasks) of a notify / notify_own event, or None if the servant index is gone."""
@@ -163,6 +233,8 @@ class Replayer:
                 trace.append(g)
             elif kind == "wait":
                 trace.append(self._wait(ev[1], ev[2](d) if callable(ev[2]) else ev[2]))
+            elif kind == "filter":
+                trace += self._filter(*ev[1:])
             elif kind == "free":
                 ids = np.asarray(ev[1], dtype=np.uint64)
                 d.free_tasks(ids)
@@ -223,6 +295,28 @@ class Replayer:
             else:  # pragma: no cover
                 raise ValueError(f"unknown event {kind!r}")
         return trace
+
+
+def with_repeats(stream: Stream, seed: int, frac: float = 0.3) -> Stream:
+    """The stream with, for a seeded `frac` of its "wait" batches, a prefix of that batch asked for again just before
+    the next "wait" event (after whatever frees and ticks lie between).  A staged Replayer decides the repeat from the
+    queue it staged for the first batch, without staging again."""
+    rng = np.random.default_rng(seed)
+    ev: list = []
+    again = None
+    for e in stream.events:
+        if e[0] == "wait":
+            if again is not None:
+                ev.append(("wait", e[1], again))
+            again = None
+            if rng.random() < frac:
+                part = float(rng.random())
+                if callable(e[2]):  # (built again when the repeat runs: the same requests, the IPs already interned)
+                    again = lambda dd, f=e[2], part=part: (lambda r: r[: max(1, int(len(r) * part))])(f(dd))  # noqa: E731
+                elif len(e[2]):
+                    again = e[2][: max(1, int(len(e[2]) * part))].copy()
+        ev.append(e)
+    return Stream(stream.name + "-repeats", ev, dict(stream.meta))
 
 
 def trace_digest(trace: Sequence[np.ndarray]) -> str:

@@ -9,11 +9,18 @@ frees them against it.  All frames that arrive within one batching window (--win
 handed to ONE yd_wire_handle_frames call, so concurrent WaitForStartingTask RPCs become one
 batched GPU solve; answers are what serving the frames one by one in arrival order would give.
 The 1 Hz expiration sweep (task_dispatcher.cc:81-82) runs from the same loop.  This is glue for
-demos and tests, not a production server: one thread, no TLS, no back-pressure."""
+demos and tests, not a production server: one thread, no TLS, no back-pressure.
+
+With --state FILE a restart keeps the scheduler's servants, leases and task ids: the state is
+imported from FILE at start if it exists, and exported to it (a temporary file, then a rename) when
+the process gets SIGINT or SIGTERM.  Nothing else goes into the file: the import rebases every time
+onto the new process's clock (include/ydstate.h), so the two processes need no common clock."""
 from __future__ import annotations
 
 import argparse
 import asyncio
+import os
+import signal
 import struct
 import sys
 import time
@@ -78,16 +85,44 @@ class Endpoint:
                 self.svc.dispatcher.on_expiration_timer(now=last_tick)
 
 
+def save_state(d: TaskDispatcher, path: str, now: float) -> None:
+    """Export the dispatcher's state to `path` atomically: a reader sees the old file or the new one."""
+    tmp = f"{path}.tmp.{os.getpid()}"
+    with open(tmp, "wb") as f:
+        f.write(d.export_state(now=now))
+        f.flush()
+        os.fsync(f.fileno())
+    os.replace(tmp, path)
+
+
 async def serve(args, ready: asyncio.Event | None = None):
     d = TaskDispatcher(args.library) if args.library else TaskDispatcher()
+    if args.state and os.path.exists(args.state):
+        with open(args.state, "rb") as f:
+            d.import_state(f.read(), now=0.0)  # now = 0 on the endpoint's clock, which starts below
     svc = SchedulerService(d, acceptable_user_tokens=args.user_tokens, acceptable_servant_tokens=args.servant_tokens,
                            min_daemon_version=args.min_daemon_version)
     ep = Endpoint(svc, args.window_ms)
     server = await asyncio.start_server(ep.client, args.host, args.port)
+    work = asyncio.gather(server.serve_forever(), ep.pump())
+    stopped = []
+    if args.state:
+        def stop():
+            save_state(d, args.state, ep.now())
+            stopped.append(True)
+            work.cancel()
+
+        loop = asyncio.get_running_loop()
+        for sig in (signal.SIGINT, signal.SIGTERM):
+            loop.add_signal_handler(sig, stop)
     if ready is not None:
         ready.set()
     async with server:
-        await asyncio.gather(server.serve_forever(), ep.pump())
+        try:
+            await work
+        except asyncio.CancelledError:
+            if not stopped:
+                raise
 
 
 def parse_args(argv=None):
@@ -99,6 +134,8 @@ def parse_args(argv=None):
     ap.add_argument("--min-daemon-version", type=int, default=0)
     ap.add_argument("--window-ms", type=float, default=1.0)
     ap.add_argument("--library", default=None, help="ydsched C-ABI library (default: the CUDA build)")
+    ap.add_argument("--state", default=None,
+                    help="state file: imported at start if it exists, exported on SIGINT / SIGTERM (include/ydstate.h)")
     return ap.parse_args(argv)
 
 

@@ -259,6 +259,12 @@ def load_library(path: os.PathLike | str | None = None) -> C.CDLL:
         fn = getattr(lib, name)  # AttributeError if the symbol is missing
         fn.restype = restype
         fn.argtypes = argtypes
+    # include/ydstate.h: the CUDA library and the port's state build (checkers/) export and import state
+    for name, restype, argtypes in STATE_PROTOTYPES:
+        fn = getattr(lib, name, None)
+        if fn is not None:
+            fn.restype = restype
+            fn.argtypes = argtypes
     # include/ydshard.h: only the CUDA library has the range-sharded multi-GPU path
     for name, restype, argtypes in SHARD_PROTOTYPES:
         fn = getattr(lib, name, None)
@@ -292,6 +298,13 @@ SHARD_PROTOTYPES = [
     ("yd_shard_free_tasks", C.c_int, [_P, _P, C.c_size_t]),
     ("yd_shard_last_stats", C.c_int, [_P, C.POINTER(yd_shard_stats)]),
 ]
+
+# Every symbol include/ydstate.h declares, and its status codes.
+STATE_PROTOTYPES = [
+    ("yd_export_state", C.c_size_t, [_P, C.c_int64, _P, C.c_size_t]),
+    ("yd_import_state", C.c_int, [_P, C.c_int64, _P, C.c_size_t]),
+]
+STATE_OK, STATE_BAD_BLOB, STATE_NOT_FRESH, STATE_CONFIG_MISMATCH, STATE_UNSUPPORTED, STATE_NO_MEMORY = 0, 1, 2, 3, 4, 5
 
 # Every symbol include/ydservice.h declares.
 SERVICE_PROTOTYPES = [

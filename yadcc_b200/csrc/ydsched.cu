@@ -35,6 +35,8 @@
 #include "tiny.cuh"
 #include "fused.cuh"
 #include "filter.cuh"
+#include "state.cuh"
+#include "ydstate_codec.inc"
 
 namespace {
 
@@ -2363,3 +2365,176 @@ size_t yd_filter_and_wait_for_starting_new_tasks(yd_sched* s, int64_t now_ns, co
 
 // ---- range-sharded queue over the GPUs of a node (include/ydshard.h) ------------------------------------
 #include "shard_host.inc"
+
+// ---- state export / import (include/ydstate.h): host side; the lease passes are in state.cuh ----------------------
+namespace {
+
+bool IsFresh(const yd_sched* s) {
+  return s->sv.empty() && s->next_id == 0 && s->lo == 0 && s->running.empty() && s->running.bucket_count() == 1 &&
+         s->envs.empty() && s->ips.size() == 1 && s->staged_n == 0;
+}
+
+// Stream-ordered temporaries (cudaMallocAsync): the export's and the import's scratch never enters a captured graph, so
+// it stays out of the grow-only buffers whose reallocation bumps g_buf_generation -- that bump would drop the captured
+// graphs and the kept class table, i.e. cost the next solve its speculation.
+void* StateTmp(yd_sched* s, size_t bytes) {
+  void* p = nullptr;
+  YD_CUDA_CHECK(cudaMallocAsync(&p, std::max<size_t>(bytes, 8), s->st));
+  return p;
+}
+
+}  // namespace
+
+extern "C" size_t yd_export_state(yd_sched* s, int64_t now_ns, uint8_t* out, size_t cap) {
+  if (s->shard) return 0;  // range-sharded handles are not exported
+  YD_CUDA_CHECK(cudaSetDevice(s->device));
+  cudaStream_t st = s->st;
+  s->SyncServantState();
+  const size_t S = s->sv.size();
+  // ever_assigned_tasks of every servant and the live-lease count of the window, one synchronisation
+  std::vector<unsigned long long> ever(S);
+  if (S) YD_CUDA_CHECK(cudaMemcpyAsync(ever.data(), s->d_ever.p, S * 8, cudaMemcpyDeviceToHost, st));
+  const uint64_t window = s->next_id - s->lo;
+  const uint32_t nb = (uint32_t)((window + 1023) / 1024);
+  uint32_t* d_off = nullptr;
+  Counters* d_sum = nullptr;
+  unsigned long long n_leases = 0;
+  if (nb) {
+    char* t = static_cast<char*>(StateTmp(s, sizeof(Counters) + size_t(nb) * 4));
+    d_sum = reinterpret_cast<Counters*>(t);
+    d_off = reinterpret_cast<uint32_t*>(t + sizeof(Counters));
+    YD_CUDA_CHECK(cudaMemsetAsync(d_sum, 0, sizeof(Counters), st));
+    yd::k_state_count<<<nb, 1024, 0, st>>>(s->ring(), d_off);
+    YD_CUDA_CHECK(cudaGetLastError());
+    // the exclusive scan of the grant path, into a scratch Counters (its total lands in ->granted)
+    yd::k_final_scan<<<1, 1024, 0, st>>>(d_off, nb, d_sum, nullptr);
+    YD_CUDA_CHECK(cudaGetLastError());
+    YD_CUDA_CHECK(cudaMemcpyAsync(&n_leases, &d_sum->granted, 8, cudaMemcpyDeviceToHost, st));
+  }
+  YD_CUDA_CHECK(cudaStreamSynchronize(st));
+
+  ydstate::StateImage im;
+  im.id_stride = s->id_stride;
+  im.id_offset = s->id_offset;
+  im.min_mem = s->min_mem;
+  im.next_task_id = yd_next_task_id(s);
+  im.envs = s->envs;
+  im.ips = s->ips;
+  im.servants.resize(S);
+  for (size_t i = 0; i != S; ++i) {
+    const ServantHost& v = s->sv[i];
+    ydstate::Servant& o = im.servants[i];
+    o.version = v.version; o.priority = v.priority; o.reason = v.reason;
+    o.nproc = v.nproc; o.load = v.load; o.max_tasks = v.max_tasks;
+    o.total_mem = v.total_mem; o.avail_mem = v.avail_mem;
+    o.expires_rel = v.expires_at - now_ns;
+    o.ever = ever[i];
+    o.observed = v.observed; o.reported = v.reported;
+    o.envs.reserve(v.envs.size());
+    for (uint32_t e : v.envs) o.envs.push_back(s->envs[e]);
+  }
+  im.n_leases = n_leases;  // (written straight into `out` below)
+  im.bucket_count = s->running.bucket_count();
+  for (auto&& [loc, v] : s->running) {
+    ydstate::Group& g = im.groups.emplace_back();
+    g.location = loc;
+    for (auto&& t : v) g.tasks.push_back(ydstate::Task{t.servant_task_id, t.task_grant_id, t.servant_location, t.task_digest});
+  }
+  size_t lease_off = 0;
+  const size_t size = ydstate::EncodeState(im, out, cap, &lease_off);
+  if (out && cap >= size && n_leases) {
+    yd::StateLease* d_rec = static_cast<yd::StateLease*>(StateTmp(s, n_leases * sizeof(yd::StateLease)));
+    yd::k_state_write<<<nb, 1024, 0, st>>>(s->ring(), (long long)now_ns, d_off, d_rec);
+    YD_CUDA_CHECK(cudaGetLastError());
+    YD_CUDA_CHECK(cudaMemcpyAsync(out + lease_off, d_rec, n_leases * sizeof(yd::StateLease), cudaMemcpyDeviceToHost, st));
+    YD_CUDA_CHECK(cudaFreeAsync(d_rec, st));
+  }
+  if (d_sum) YD_CUDA_CHECK(cudaFreeAsync(d_sum, st));
+  YD_CUDA_CHECK(cudaStreamSynchronize(st));
+  return size;
+}
+
+extern "C" int yd_import_state(yd_sched* s, int64_t now_ns, const uint8_t* blob, size_t len) {
+  if (s->shard) return YD_STATE_UNSUPPORTED;
+  if (!IsFresh(s)) return YD_STATE_NOT_FRESH;
+  ydstate::StateImage im;
+  if (int rc = ydstate::DecodeState(blob, len, &im)) return rc;
+  if (im.id_stride != s->id_stride || im.id_offset != s->id_offset || im.min_mem != s->min_mem) return YD_STATE_CONFIG_MISMATCH;
+  YD_CUDA_CHECK(cudaSetDevice(s->device));
+  cudaStream_t st = s->st;
+  auto local = [&](uint64_t ext) { return (ext - im.id_offset) / im.id_stride; };
+  const uint64_t next_id = local(im.next_task_id);
+  const uint64_t lo = im.leases.empty() ? next_id : local(im.leases.front().id);
+  // The ring is sized from the oldest live id, as EnsureRing would have grown it (DecodeState bounds the window by
+  // kMaxWindow, so none of this overflows); a valid export that cannot fit the device's free memory now is refused.
+  uint64_t ring_cap = 1ull << 16;
+  while (ring_cap < (next_id - lo) * 2) ring_cap <<= 1;
+  size_t free_b = 0, total_b = 0;
+  YD_CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
+  if (ring_cap * 16 + im.leases.size() * sizeof(yd::StateLease) > free_b) return YD_STATE_NO_MEMORY;
+
+  // host side: exactly what KeepServantAlive, the interning calls and the bookkeeper would have built
+  s->envs = im.envs;
+  s->ips = im.ips;
+  s->env_ids.clear();
+  s->ip_ids.clear();
+  for (uint32_t i = 0; i != s->envs.size(); ++i) s->env_ids.emplace(s->envs[i], i);
+  for (uint32_t i = 0; i != s->ips.size(); ++i) s->ip_ids.emplace(s->ips[i], i);
+  const uint32_t S = (uint32_t)im.servants.size();
+  std::vector<unsigned long long> ever(S);
+  for (uint32_t i = 0; i != S; ++i) {
+    const ydstate::Servant& v = im.servants[i];
+    ServantHost& rec = s->sv.emplace_back();
+    rec.version = v.version; rec.priority = v.priority; rec.reason = v.reason;
+    rec.observed = v.observed; rec.reported = v.reported;
+    for (auto&& e : v.envs) rec.envs.push_back(s->InternEnv(e));
+    rec.nproc = v.nproc; rec.load = v.load; rec.max_tasks = v.max_tasks;
+    rec.total_mem = v.total_mem; rec.avail_mem = v.avail_mem;
+    rec.discovered_at = now_ns;
+    rec.expires_at = now_ns + v.expires_rel;
+    s->loc2pos.emplace(rec.observed, i);
+    ever[i] = v.ever;
+  }
+  // the bookkeeper's iteration order: same bucket count, groups inserted last-first (ydstate.h)
+  if (im.bucket_count != 1) s->running.rehash(im.bucket_count);
+  for (auto g = im.groups.rbegin(); g != im.groups.rend(); ++g) {
+    std::vector<RunningRec> v;
+    for (auto&& t : g->tasks) v.push_back(RunningRec{t.servant_task_id, t.task_grant_id, t.servant_location, t.task_digest});
+    s->running.emplace(g->location, std::move(v));
+  }
+  s->topo_dirty = s->facts_dirty = s->order_dirty = true;  // the first solve rebuilds topology, facts and slot order
+
+  // device side: servant state, the ring, the counters
+  if (S) {
+    s->d_run.ensure(size_t(S) * 4);
+    s->d_ever.ensure(size_t(S) * 8);
+    YD_CUDA_CHECK(cudaMemsetAsync(s->d_run.p, 0, size_t(S) * 4, st));
+    YD_CUDA_CHECK(cudaMemcpyAsync(s->d_ever.p, ever.data(), size_t(S) * 8, cudaMemcpyHostToDevice, st));
+  }
+  s->S_dev = S;
+  s->d_t_exp.release(); s->d_t_srv.release(); s->d_t_flags.release();
+  s->ring_cap = 0;
+  s->lo = lo;
+  s->next_id = next_id;
+  s->EnsureRing(0);
+  const size_t n = im.leases.size();
+  uint64_t zombies = 0;
+  for (auto&& l : im.leases) zombies += (l.flags & YD_STATE_LEASE_ZOMBIE) != 0;
+  if (n) {
+    yd::StateLease* d_rec = static_cast<yd::StateLease*>(StateTmp(s, n * sizeof(yd::StateLease)));
+    YD_CUDA_CHECK(cudaMemcpyAsync(d_rec, im.leases.data(), n * sizeof(yd::StateLease), cudaMemcpyHostToDevice, st));
+    yd::k_state_scatter<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_rec, (uint32_t)n, s->ring(), (long long)now_ns,
+                                                                    s->d_run.as<uint32_t>());
+    YD_CUDA_CHECK(cudaGetLastError());
+    YD_CUDA_CHECK(cudaFreeAsync(d_rec, st));
+  }
+  Counters* c = s->h_counters.as<Counters>();
+  memset(c, 0, sizeof(Counters));
+  c->alive = n;
+  c->zombies = zombies;
+  c->min_live = ~0ull;
+  YD_CUDA_CHECK(cudaMemcpyAsync(s->d_counters.p, c, sizeof(Counters), cudaMemcpyHostToDevice, st));
+  YD_CUDA_CHECK(cudaStreamSynchronize(st));
+  s->zombies_ub = zombies;
+  return YD_STATE_OK;
+}

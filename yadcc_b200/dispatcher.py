@@ -73,6 +73,18 @@ class RunningTask:
     task_digest: str = ""
 
 
+class StateError(RuntimeError):
+    """yd_import_state refused an export; `code` is one of _abi.STATE_* (ydstate.h)."""
+
+    NAMES = {1: "malformed export", 2: "the handle is not fresh", 3: "the export's config differs from the handle's",
+             4: "range-sharded handles have no state export",
+             5: "the export's lease window does not fit the device's free memory now"}
+
+    def __init__(self, code: int):
+        super().__init__(f"yd_import_state: {self.NAMES.get(code, code)}")
+        self.code = code
+
+
 def _ns(seconds: float | int) -> int:
     return int(round(seconds * 1_000_000_000))
 
@@ -498,6 +510,35 @@ class TaskDispatcher:
             return None
         return RunningTask(int(t.servant_task_id), int(t.task_grant_id), (t.servant_location or b"").decode(),
                            (t.task_digest or b"").decode())
+
+    # -- state export / import (include/ydstate.h) --------------------------
+    def _state_fn(self, name: str):
+        fn = getattr(self._lib, name, None)
+        if fn is None:
+            raise NotImplementedError(f"{self._lib._yd_path} does not export {name}")
+        return fn
+
+    def export_state(self, now: float = 0.0, *, now_ns: int | None = None) -> bytes:
+        """The handle's decision state (servants, leases, next task id, running-task bookkeeping, intern
+        tables) in the versioned format of ydstate.h, times relative to `now`."""
+        fn = self._state_fn("yd_export_state")
+        t = now_ns if now_ns is not None else _ns(now)
+        n = fn(self._h, t, None, 0)
+        if n == 0:
+            raise StateError(_abi.STATE_UNSUPPORTED)
+        buf = C.create_string_buffer(n)
+        m = fn(self._h, t, buf, n)
+        assert m == n, (m, n)
+        return buf.raw
+
+    def import_state(self, blob: bytes, now: float = 0.0, *, now_ns: int | None = None) -> None:
+        """Load an export into this handle, which must be fresh (no call since construction).  Times are
+        rebased onto `now`.  Raises StateError with the ydstate.h status code if the export is refused."""
+        fn = self._state_fn("yd_import_state")
+        data = bytes(blob)
+        rc = fn(self._h, now_ns if now_ns is not None else _ns(now), data, len(data))
+        if rc != _abi.STATE_OK:
+            raise StateError(rc)
 
     # -- introspection -----------------------------------------------------
     def num_servants(self) -> int:

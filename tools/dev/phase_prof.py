@@ -15,7 +15,7 @@ from bench import build_workload
 from yadcc_b200 import STATUS_GRANTED, TaskDispatcher, pack_requests, unpack_grants
 
 KINDS = {1: "request tile", 2: "slot tile", 3: "class item"}
-WORDS = 8  # fused.cuh: kProfBlockWords
+WORDS = 12  # fused.cuh: kProfBlockWords
 
 
 def captured(fn):
@@ -57,6 +57,14 @@ def block_table(line, event_us):
         ("phase B", (b[:, 6] - b[:, 5]) / 1e3),
         ("end of B", (b[:, 6] - t0) / 1e3),
     ]
+    # phase B of the block's first request tile, link by link (blocks without a request tile leave words 8..10 at 0)
+    tiled = b[b[:, 10] != 0]
+    if len(tiled):
+        rows += [
+            (f"B: tables, n={len(tiled)}", (tiled[:, 8] - tiled[:, 5]) / 1e3),
+            ("B: selection", (tiled[:, 9] - tiled[:, 8]) / 1e3),
+            ("B: final_tile", (tiled[:, 10] - tiled[:, 9]) / 1e3),
+        ]
     span = (max(b[:, 6].max(), last_end) - t0) / 1e3
     head = (f"    {G} blocks; kernel span {span:.1f} us (first start .. last block done, report and clean-up included), "
             f"event {event_us:.1f} us, launch + drain {event_us - span:.1f} us")

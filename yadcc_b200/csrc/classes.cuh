@@ -437,9 +437,43 @@ constexpr uint32_t kListChunk = 64;
 // kernel, whichever of the two it calls).
 __shared__ uint32_t s_count_bal[kListChunk][32];
 
+// Solo solves (fused.cuh) select a list's k-th member straight from per-tile MEMBER LISTS, written where the ballots are
+// made: members[(tile * cls_bound + c) * kListTile + j] = the registry position of the j-th member of list c inside slot
+// tile `tile` (j = the member's rank in the tile's list: members of the list in lower warps + in lower lanes of its
+// warp).  A solo solve's components with requests hold one class each, so a slot is in one list at most.
+__device__ __forceinline__ size_t list_member_index(uint32_t tile, uint32_t c, uint32_t cls_bound) {
+  return (size_t(tile) * cls_bound + c) * kListTile;
+}
+
+// The counts of lists c0 .. c1 in this tile from the chunk's ballots in s_count_bal (warp c - c0 takes list c).
+// `prefix`: each ballot word is then replaced by the list's members in the lower warps (the member lists' offsets).
+__device__ __forceinline__ void list_chunk_counts(uint32_t c0, uint32_t c1, uint32_t tile, uint32_t n_tiles,
+                                                  uint32_t* __restrict__ counts, bool prefix) {
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (uint32_t c = c0 + warp; c < c1; c += 32) {
+    const uint32_t v = __popc(s_count_bal[c - c0][lane]);
+    uint32_t cnt;
+    if (prefix) {
+      uint32_t x = v;
+#pragma unroll
+      for (int s = 1; s < 32; s <<= 1) {
+        const uint32_t y = __shfl_up_sync(0xffffffffu, x, s);
+        if (lane >= s) x += y;
+      }
+      s_count_bal[c - c0][lane] = x - v;
+      cnt = __shfl_sync(0xffffffffu, x, 31);
+    } else {
+      cnt = __reduce_add_sync(0xffffffffu, v);
+    }
+    if (lane == 0) counts[c * n_tiles + tile] = cnt;
+  }
+}
+
+// `members`: solo solves only (see list_member_index), else null.
 __device__ __forceinline__ void list_count_tile(uint32_t tile, uint32_t m, const SlotDecode& d, const TopoView& t,
                                                 const ClassTable& ct, const ServantArrays& sv, uint32_t n_tiles,
-                                                uint32_t* __restrict__ counts, uint32_t* __restrict__ balg) {
+                                                uint32_t* __restrict__ counts, uint32_t* __restrict__ balg,
+                                                uint32_t* __restrict__ members) {
   auto& bal = s_count_bal;
   const uint32_t ncls = min(ct.meta[0], ct.cls_bound);
   const uint32_t nmerge = min(ct.meta[2], ct.cls_bound - ncls);
@@ -452,6 +486,7 @@ __device__ __forceinline__ void list_count_tile(uint32_t tile, uint32_t m, const
   bool any = false;  // my servant is eligible for some class of its component
   for (uint32_t c0 = 0; c0 < ncls + nmerge; c0 += kListChunk) {
     const uint32_t c1 = min(c0 + kListChunk, ncls + nmerge);
+    uint32_t my_c = kNone, my_bal = 0;  // (members) my slot's class list in this chunk, and its ballot
     for (uint32_t c = c0; c < c1; ++c) {
       bool in;
       if (c < ncls) {  // class list: eligibility (cc:316-344)
@@ -462,11 +497,15 @@ __device__ __forceinline__ void list_count_tile(uint32_t tile, uint32_t m, const
       }
       const uint32_t b = __ballot_sync(0xffffffffu, in);
       if (lane == 0) { bal[c - c0][warp] = b; my_row[c * 32 + warp] = b; }
+      if (in && c < ncls) { my_c = c; my_bal = b; }
     }
     __syncthreads();
-    for (uint32_t c = c0 + warp; c < c1; c += 32) {
-      const uint32_t cnt = __reduce_add_sync(0xffffffffu, (uint32_t)__popc(bal[c - c0][lane]));
-      if (lane == 0) counts[c * n_tiles + tile] = cnt;
+    list_chunk_counts(c0, c1, tile, n_tiles, counts, members != nullptr);
+    if (members) {
+      __syncthreads();
+      if (my_c != kNone) {
+        members[list_member_index(tile, my_c, ct.cls_bound) + bal[my_c - c0][warp] + __popc(my_bal & ((1u << lane) - 1))] = pos;
+      }
     }
     __syncthreads();  // the ballots have been consumed
   }
@@ -479,11 +518,12 @@ __device__ __forceinline__ void list_count_tile(uint32_t tile, uint32_t m, const
 // of its component, if it holds the class's digest; written with the table), if the servant's version is high enough.
 // So: three gathers per slot (run, kept_sv, version) instead of four to five, one test, and the lanes of a warp grouped
 // by list (__match_any_sync) instead of one ballot per class.  s_mv: the classes' min_versions in shared memory, loaded
-// by the block's first call (`facts`).
+// by the block's first call (`facts`).  It writes the member lists (list_member_index), not the ballot words: the
+// speculative solve selects from the member lists alone.
 __device__ __forceinline__ void list_count_tile_kept(uint32_t tile, uint32_t m, uint32_t ncls, const SlotDecode& d,
                                                      const ClassTable& ct, const ServantArrays& sv,
                                                      const uint32_t* __restrict__ kept_sv, uint32_t n_tiles,
-                                                     uint32_t* __restrict__ counts, uint32_t* __restrict__ balg,
+                                                     uint32_t* __restrict__ counts, uint32_t* __restrict__ members,
                                                      uint32_t* s_mv, bool& facts) {
   auto& bal = s_count_bal;
   uint32_t* const bal_flat = &bal[0][0];
@@ -500,7 +540,6 @@ __device__ __forceinline__ void list_count_tile_kept(uint32_t tile, uint32_t m, 
   facts = true;
   // a slot outside its row, one the servant has filled already, or a servant below the class's min_version: no list
   if (rec.x == kNone || rec.y < run || cls >= ncls || ver < s_mv[cls]) cls = kNone;
-  uint32_t* my_row = balg + size_t(tile) * ct.cls_bound * 32;
   for (uint32_t c0 = 0; c0 < ncls; c0 += kListChunk) {
     const uint32_t c1 = min(c0 + kListChunk, ncls);
     for (uint32_t k = tid; k < (c1 - c0) * 32; k += kListTile) bal_flat[k] = 0;
@@ -509,10 +548,10 @@ __device__ __forceinline__ void list_count_tile_kept(uint32_t tile, uint32_t m, 
     const uint32_t peers = __match_any_sync(0xffffffffu, key);  // = the ballot of list `key` in this warp
     if (key != kNone && lane == (uint32_t)(__ffs(peers) - 1)) bal[key - c0][warp] = peers;
     __syncthreads();
-    for (uint32_t k = tid; k < (c1 - c0) * 32; k += kListTile) my_row[c0 * 32 + k] = bal_flat[k];
-    for (uint32_t c = c0 + warp; c < c1; c += 32) {
-      const uint32_t cnt = __reduce_add_sync(0xffffffffu, (uint32_t)__popc(bal[c - c0][lane]));
-      if (lane == 0) counts[c * n_tiles + tile] = cnt;
+    list_chunk_counts(c0, c1, tile, n_tiles, counts, true);
+    __syncthreads();
+    if (key != kNone) {
+      members[list_member_index(tile, key, ct.cls_bound) + bal[key - c0][warp] + __popc(peers & ((1u << lane) - 1))] = rec.x;
     }
     __syncthreads();  // the ballots have been consumed
   }
@@ -522,7 +561,7 @@ __global__ void __launch_bounds__(kListTile) k_list_count(const unsigned long lo
                                                           TopoView t, ClassTable ct, ServantArrays sv,
                                                           uint32_t n_tiles, uint32_t* __restrict__ counts,
                                                           uint32_t* __restrict__ balg) {
-  list_count_tile(blockIdx.x, (uint32_t)*m_ptr, d, t, ct, sv, n_tiles, counts, balg);
+  list_count_tile(blockIdx.x, (uint32_t)*m_ptr, d, t, ct, sv, n_tiles, counts, balg, nullptr);
 }
 
 // counts[] has been exclusive-scanned over (class-major, tile-minor).

@@ -112,6 +112,7 @@ struct FusedArgs {
   uint32_t* rank_cnt;
   uint32_t* list_cnt;
   uint32_t* list_bal;
+  uint32_t* members;  // solo: the per-tile member lists (classes.cuh: list_member_index)
   uint2* list;
   uint32_t list_cap;
   uint2* rq;
@@ -136,9 +137,10 @@ struct FusedArgs {
 // YDSCHED_FUSED_PROF: block 0 stamps every phase boundary into prof[0 .. 9).  The speculative variant also stamps, per
 // block b, prof[kProfHead + b * kProfBlockWords + k]: k = 0 start, 1..3 end of its first three items of phase A, 4
 // barrier arrival, 5 departure, 6 end of phase B; word 7 = the kinds of those items (4 bits each, FusedItem) | the
-// number of items << 16.
+// number of items << 16; then, for the block's first request tile of phase B, 8 end of the table build (list offsets,
+// request prefixes, base), 9 end of the selection, 10 end of final_tile; word 11 is unused.
 constexpr uint32_t kProfHead = 16;
-constexpr uint32_t kProfBlockWords = 8;
+constexpr uint32_t kProfBlockWords = 12;
 constexpr uint32_t kProfMaxItems = 3;
 enum FusedItem : uint32_t { kItemRequests = 1, kItemSlots = 2, kItemClass = 3 };
 
@@ -208,6 +210,23 @@ __device__ __forceinline__ void fused_barrier(uint32_t* bar, uint32_t epoch) {
     while (fused_ld_acquire(&bar[0]) < want) {}
   }
   __syncthreads();
+}
+// The same, with a flag raised by any block delivered with the release: a block that raises it arrives with
+// kBarFlag + 1 instead of 1, so the count is the low bits of the word and the flags the high bits; the word each block
+// acquires when it leaves holds every block's arrival.  Returns whether any block raised it -- no load after the wait.
+constexpr uint32_t kBarFlag = 1u << 24;  // (grids of fewer than 2^24 blocks, fewer than 256 flags)
+__device__ __forceinline__ bool fused_barrier_any(uint32_t* bar, uint32_t epoch, bool flag) {
+  __shared__ uint32_t s_any;
+  const bool mine = __syncthreads_or(flag);
+  if (threadIdx.x == 0) {
+    fused_atom_add_acq_rel(&bar[0], mine ? kBarFlag + 1u : 1u);
+    const uint32_t want = epoch * gridDim.x;
+    uint32_t v;
+    while (((v = fused_ld_acquire(&bar[0])) & (kBarFlag - 1u)) < want) {}
+    s_any = v >> 24;
+  }
+  __syncthreads();
+  return s_any != 0;
 }
 // "I am done": true in the block that finishes last -- it has acquired everything the grid wrote.
 __device__ __forceinline__ bool fused_done_last(uint32_t* bar) {
@@ -328,87 +347,33 @@ __device__ __forceinline__ void fused_scan_flat(uint32_t* __restrict__ data, uin
   }
 }
 
-// Solo solves skip the compacted lists: the request with FIFO rank k in class c takes the k-th member of c's list, and
-// that member is found straight from what the count phase left behind -- the scanned (class, tile) offsets (`loff`, in
-// shared memory when they fit) name the slot tile, the tile's membership ballot (32 words) names the slot, the kept
-// order's record names the servant.  Returns the verdict: a REGISTRY POSITION, kResTimeout or kResEnvNotFound.
-__device__ __forceinline__ uint32_t fused_select(uint32_t q, const FusedArgs& a, const uint32_t* __restrict__ loff) {
-  const uint32_t c = a.rcls[q];
-  if (c == kNone) return kResEnvNotFound;           // unknown digest, or one nobody holds
-  if (a.ct.cls_nelig[c] == 0) return kResEnvNotFound;  // cc:105-108
-  const uint32_t rank = a.rank_cnt[c * a.n_rtiles + q / kRankTile] - a.rank_cnt[c * a.n_rtiles] + a.rrank[q];
-  const uint32_t* row = loff + c * a.n_ltiles;
-  const uint32_t lb = row[0], le = row[a.n_ltiles];
-  if (rank >= le - lb) return kResTimeout;            // cc:116-118
-  const uint32_t target = lb + rank;
+// Solo solves skip the compacted lists: the request of class c (not kNone) with class rank `rank` (its FIFO rank among
+// the batch's class-c requests) takes the rank-th member of c's list, found straight from what the count phase left
+// behind: class c's (class, tile) offsets (`rows + c * stride`: one word per slot tile + the end, in shared memory when
+// they fit) name the slot tile and the rank inside it, and the tile's member list names the servant -- one load.
+// `nelig`: the classes' eligible-servant counts.  Returns the verdict: a REGISTRY POSITION, kResTimeout or
+// kResEnvNotFound.
+__device__ __forceinline__ uint32_t fused_select(uint32_t c, uint32_t rank, const FusedArgs& a,
+                                                 const uint32_t* __restrict__ nelig, const uint32_t* __restrict__ rows,
+                                                 uint32_t stride) {
+  if (nelig[c] == 0) return kResEnvNotFound;  // cc:105-108
+  const uint32_t* row = rows + c * stride;
+  const uint32_t target = row[0] + rank;
+  if (target >= row[a.n_ltiles]) return kResTimeout;  // cc:116-118
   uint32_t lo = 0, hi = a.n_ltiles;                   // the last tile whose offset is <= target holds it
   while (hi - lo > 1) {
     const uint32_t mid = (lo + hi) >> 1;
     if (row[mid] <= target) lo = mid; else hi = mid;
   }
-  uint32_t j = target - row[lo];                      // the j-th member inside tile lo
-  const uint4* words = reinterpret_cast<const uint4*>(a.list_bal + (size_t(lo) * a.ct.cls_bound + c) * 32);
-  uint32_t w = 0, word = 0;
-  bool found = false;
-#pragma unroll 1
-  for (uint32_t v = 0; v < 8 && !found; ++v) {
-    const uint4 x = words[v];
-    const uint32_t xs[4] = {x.x, x.y, x.z, x.w};
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      if (!found) {
-        const uint32_t p = __popc(xs[k]);
-        if (j < p) { found = true; w = v * 4 + k; word = xs[k]; }
-        else j -= p;
-      }
-    }
-  }
-  const uint32_t bit = __fns(word, 0, (int)j + 1);
-  return a.dec.rec[lo * kListTile + w * 32 + bit].x;
+  return a.members[list_member_index(lo, c, a.ct.cls_bound) + (target - row[lo])];
 }
 
-// The same with block-local tables built from the RAW counts (no scan by a leader): `rows` = per class the exclusive
-// offsets of its slot tiles + its total (n_ltiles + 1 words per class), `rpre[c]` = class-c requests in the request tiles
-// before this one; c / rank = the request's class and its rank among the class's requests of its tile.
-__device__ __forceinline__ uint32_t fused_select_lite(uint32_t c, uint32_t rank, const FusedArgs& a,
-                                                       const uint32_t* __restrict__ rows, const uint32_t* __restrict__ rpre) {
-  if (c == kNone) return kResEnvNotFound;
-  if (a.ct.cls_nelig[c] == 0) return kResEnvNotFound;  // cc:105-108
-  const uint32_t target = rpre[c] + rank;
-  const uint32_t* row = rows + c * (a.n_ltiles + 1);
-  if (target >= row[a.n_ltiles]) return kResTimeout;   // cc:116-118
-  uint32_t lo = 0, hi = a.n_ltiles;
-  while (hi - lo > 1) {
-    const uint32_t mid = (lo + hi) >> 1;
-    if (row[mid] <= target) lo = mid; else hi = mid;
-  }
-  uint32_t j = target - row[lo];
-  const uint4* words = reinterpret_cast<const uint4*>(a.list_bal + (size_t(lo) * a.ct.cls_bound + c) * 32);
-  uint32_t w = 0, word = 0;
-  bool found = false;
-#pragma unroll 1
-  for (uint32_t v = 0; v < 8 && !found; ++v) {
-    const uint4 x = words[v];
-    const uint32_t xs[4] = {x.x, x.y, x.z, x.w};
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      if (!found) {
-        const uint32_t p = __popc(xs[k]);
-        if (j < p) { found = true; w = v * 4 + k; word = xs[k]; }
-        else j -= p;
-      }
-    }
-  }
-  const uint32_t bit = __fns(word, 0, (int)j + 1);
-  return a.dec.rec[lo * kListTile + w * 32 + bit].x;
-}
-
-// Task ids of a solo solve in closed form.  The selections above grant the class-c request with class rank k exactly
+// Task ids of a solo solve in closed form.  The selection above grants the class-c request with class rank k exactly
 // when cls_nelig[c] != 0 && k < L_c (L_c = the length of c's list), so of the `before` class-c requests in the tiles
 // before a tile, min(before, L_c) were granted; summed over the classes that is the tile's first FIFO ordinal.  Every
 // block derives it from the count matrices it already holds: no tile waits for another.
-__device__ __forceinline__ uint32_t fused_class_grants(const FusedArgs& a, uint32_t c, uint32_t before, uint32_t len) {
-  return a.ct.cls_nelig[c] != 0 ? min(before, len) : 0u;
+__device__ __forceinline__ uint32_t fused_class_grants(uint32_t nelig, uint32_t before, uint32_t len) {
+  return nelig != 0 ? min(before, len) : 0u;
 }
 
 // Request q = tile * 1024 + thread (a block of 1024 threads): its digest id, min_version and requestor IP; false beyond
@@ -462,7 +427,7 @@ __global__ void __launch_bounds__(1024, 1) k_fused_front(FusedArgs a) {
     if (blockIdx.x == 0) a.prof[0] = t0;
     if (a.spec) {
       fused_bstamp(a, 0, t0);
-      fused_bstamp(a, 7, 0);
+      for (uint32_t k = 7; k < kProfBlockWords; ++k) fused_bstamp(a, k, 0);
     }
   }
   if (tid == 0) {
@@ -526,7 +491,7 @@ __global__ void __launch_bounds__(1024, 1) k_fused_front(FusedArgs a) {
         else miss = true;  // (more request tiles than two per block: the host does not speculate on such batches)
         kind = kItemRequests;
       } else if (it < nb_live + lt_live) {
-        list_count_tile_kept(it - nb_live, m, ncls, a.dec, a.ct, a.sv, a.kept_sv, a.n_ltiles, a.list_cnt, a.list_bal,
+        list_count_tile_kept(it - nb_live, m, ncls, a.dec, a.ct, a.sv, a.kept_sv, a.n_ltiles, a.list_cnt, a.members,
                              s_cls_mv, facts);
         kind = kItemSlots;
       } else {
@@ -543,14 +508,15 @@ __global__ void __launch_bounds__(1024, 1) k_fused_front(FusedArgs a) {
     // slot tiles beyond the table's end hold no members (the lists' row scans below read them; nothing re-zeroes them)
     const uint32_t tail = a.n_ltiles - lt_live;
     for (uint32_t i = blockIdx.x * 1024 + tid; i < nlists * tail; i += G * 1024) a.list_cnt[(i / tail) * a.n_ltiles + lt_live + i % tail] = 0;
-    if (__syncthreads_or(miss) && tid == 0) atomicExch(&a.ct.meta[1], kFlagSpecMiss);
+    // (meta[1] is for the report; the barrier tells the blocks)
+    if (__any_sync(0xffffffffu, miss) && (tid & 31) == 0) atomicExch(&a.ct.meta[1], kFlagSpecMiss);
     lite = true;  // (the host speculates only when the lists' offsets fit in shared memory)
     fused_stamp(a, 1);
     fused_bstamp(a, 4, fused_now());
-    fused_barrier(a.bar, 1);
+    const bool missed = fused_barrier_any(a.bar, 1, miss);
     fused_stamp(a, 2);
     fused_bstamp(a, 5, fused_now());
-    if (*reinterpret_cast<volatile uint32_t*>(&a.ct.meta[1]) != 0) {
+    if (missed) {
       // nothing is decided: the last block reports and leaves the scratch clean (the kept table too) for the replay
       if (fused_done_last(a.bar)) {
         fused_report(a, s_seq, 0);
@@ -591,7 +557,7 @@ __global__ void __launch_bounds__(1024, 1) k_fused_front(FusedArgs a) {
     const uint32_t items = lt_live + a.n_rtiles + ncls;
     for (uint32_t it = blockIdx.x; it < items; it += G) {
       if (it < lt_live) {
-        list_count_tile(it, m, a.dec, a.t, a.ct, a.sv, a.n_ltiles, a.list_cnt, a.list_bal);
+        list_count_tile(it, m, a.dec, a.t, a.ct, a.sv, a.n_ltiles, a.list_cnt, a.list_bal, a.solo ? a.members : nullptr);
       } else if (it < lt_live + a.n_rtiles) {
         const uint32_t tile = it - lt_live;
         if (tile < nb_live) {
@@ -640,49 +606,93 @@ __global__ void __launch_bounds__(1024, 1) k_fused_front(FusedArgs a) {
   ring.next = s_dyn.ring_next;
   void* const out = s_zc_out ? reinterpret_cast<void*>(s_zc_out) : a.out;
   if (a.solo && lite) {
-    // every component with requests is data-parallel: no lists, the members are selected from the ballots; the tables
-    // the selection searches are built here, per block, from the raw (class, tile) counts
-    __shared__ uint32_t s_rpre[kMaxClasses];
-    const uint32_t lane = tid & 31, warp = tid >> 5, stride = a.n_ltiles + 1;
-    for (uint32_t c = warp; c < nlists; c += 32) {  // row-local exclusive offsets of class c's slot tiles + its total
-      uint32_t running = 0;
-      for (uint32_t t0 = 0; t0 < a.n_ltiles; t0 += 32) {
-        const uint32_t t = t0 + lane;
-        const uint32_t v = t < a.n_ltiles ? a.list_cnt[c * a.n_ltiles + t] : 0u;
-        uint32_t x = v;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-          const uint32_t y = __shfl_up_sync(0xffffffffu, x, d);
-          if (lane >= d) x += y;
-        }
-        if (t < a.n_ltiles) s_loff[c * stride + t] = running + x - v;
-        running += __shfl_sync(0xffffffffu, x, 31);
-      }
-      if (lane == 0) s_loff[c * stride + a.n_ltiles] = running;
-    }
+    // every component with requests is data-parallel: no lists, each request's member is picked from the per-tile member
+    // lists; the tables the selection searches are built here, per block, from the raw (class, tile) counts.  Every load
+    // of those tables, the request's class and rank (not speculative) and its lease fields (final_tile) are issued before
+    // the first wait: one round trip to L2, then shared memory, then the member load.
+    __shared__ uint32_t s_rpre[kMaxClasses];   // class-c requests in the request tiles before this one
+    __shared__ uint32_t s_nelig[kMaxClasses];  // cls_nelig
+    __shared__ uint32_t s_base;                // grants of the request tiles before this one
+    const uint32_t lane = tid & 31, warp = tid >> 5, stride = a.n_ltiles + 1, cells = nlists * a.n_ltiles;
     for (uint32_t tile = blockIdx.x, k = 0; tile < nb_live; tile += G, ++k) {
-      __syncthreads();  // (s_loff is complete; s_rpre of the previous tile has been consumed)
-      uint32_t before = 0;  // (lane 0 of each warp) grants of its classes in the tiles before this one
-      for (uint32_t c = warp; c < ncls; c += 32) {  // class-c requests in the tiles before this one
-        uint32_t sum = 0;
-        for (uint32_t t = lane; t < tile; t += 32) sum += a.rank_cnt[c * a.n_rtiles + t];
-        sum = __reduce_add_sync(0xffffffffu, sum);
-        if (lane == 0) {
-          s_rpre[c] = sum;
-          before += fused_class_grants(a, c, sum, s_loff[c * stride + a.n_ltiles]);
+      const uint32_t q = tile * 1024 + tid;
+      uint32_t c = kNone, rank = 0, lflags = 0;  // rank: among the class's requests of this tile
+      long long lexp = 0;
+      if (q < n) {
+        rv.lease(q, lflags, lexp);
+        if (a.spec) {
+          const uint32_t cr = k == 0 ? spec_cr0 : spec_cr1;
+          if ((cr & 0xffffu) != 0xffffu) { c = cr & 0xffffu; rank = cr >> 16; }
+        } else {
+          c = a.rcls[q];
+          rank = a.rrank[q];
         }
       }
-      const uint32_t base = fused_block_sum(before);  // (also the barrier that publishes s_rpre)
-      const uint32_t q = tile * 1024 + tid;
-      uint32_t r = kResEnvNotFound;
-      if (q < n && a.spec) {
-        const uint32_t cr = k == 0 ? spec_cr0 : spec_cr1, c = cr & 0xffffu;
-        r = fused_select_lite(c == 0xffffu ? kNone : c, cr >> 16, a, s_loff, s_rpre);
-      } else if (q < n) {
-        r = fused_select_lite(a.rcls[q], a.rrank[q], a, s_loff, s_rpre);
+      uint32_t cnt0 = 0, nelig = 0;  // (first tile) this thread's first (class, slot tile) count, class tid's cls_nelig
+      if (k == 0) {
+        if (tid < cells) cnt0 = a.list_cnt[tid];
+        if (tid < ncls) nelig = a.ct.cls_nelig[tid];
       }
-      if (a.packed_out) final_tile<true, true, true>(tile, nb_live - 1, r, n, now_ns, rv, nullptr, a.comp_sv, ring, out, a.counters, a.sv.run, a.sv.ever, base);
-      else final_tile<false, true, true>(tile, nb_live - 1, r, n, now_ns, rv, nullptr, a.comp_sv, ring, out, a.counters, a.sv.run, a.sv.ever, base);
+      if (tid == 0) s_base = 0;
+      for (uint32_t cc = warp; cc < ncls; cc += 32) {  // class-cc requests in the tiles before this one
+        uint32_t sum = 0;
+        for (uint32_t t0 = 0; t0 < tile; t0 += 4 * 32) {
+          uint32_t v[4];
+#pragma unroll
+          for (int u = 0; u < 4; ++u) {
+            const uint32_t t = t0 + u * 32 + lane;
+            v[u] = t < tile ? a.rank_cnt[cc * a.n_rtiles + t] : 0u;
+          }
+          sum += v[0] + v[1] + v[2] + v[3];
+        }
+        sum = __reduce_add_sync(0xffffffffu, sum);
+        if (lane == 0) s_rpre[cc] = sum;
+      }
+      if (k == 0) {
+        if (tid < cells) s_loff[(tid / a.n_ltiles) * stride + tid % a.n_ltiles] = cnt0;
+        for (uint32_t i = tid + 1024; i < cells; i += 1024) s_loff[(i / a.n_ltiles) * stride + i % a.n_ltiles] = a.list_cnt[i];
+        if (tid < ncls) s_nelig[tid] = nelig;
+      }
+      __syncthreads();
+      // (first tile) class cc's row of counts -> row-local exclusive offsets of its slot tiles + its total, in place;
+      // then the class's grants in the request tiles before this one
+      for (uint32_t cc = warp; cc < nlists; cc += 32) {
+        uint32_t* row = s_loff + cc * stride;
+        uint32_t running = 0;
+        if (k == 0) {
+          for (uint32_t t0 = 0; t0 < a.n_ltiles; t0 += 32) {
+            const uint32_t t = t0 + lane;
+            const uint32_t v = t < a.n_ltiles ? row[t] : 0u;
+            uint32_t x = v;
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) {
+              const uint32_t y = __shfl_up_sync(0xffffffffu, x, d);
+              if (lane >= d) x += y;
+            }
+            if (t < a.n_ltiles) row[t] = running + x - v;
+            running += __shfl_sync(0xffffffffu, x, 31);
+          }
+          if (lane == 0) row[a.n_ltiles] = running;
+        } else {
+          running = row[a.n_ltiles];
+        }
+        if (lane == 0 && cc < ncls) {
+          const uint32_t g = fused_class_grants(s_nelig[cc], s_rpre[cc], running);
+          if (g) atomicAdd(&s_base, g);
+        }
+      }
+      __syncthreads();
+      const uint32_t base = s_base;
+      const bool stamp = a.prof && a.spec && k == 0;
+      if (stamp) fused_bstamp(a, 8, fused_now());
+      const uint32_t r = c != kNone ? fused_select(c, s_rpre[c] + rank, a, s_nelig, s_loff, stride) : kResEnvNotFound;
+      if (stamp) {
+        __syncthreads();  // (every selection of the tile is done)
+        fused_bstamp(a, 9, fused_now());
+      }
+      if (a.packed_out) final_tile<true, true, true, true>(tile, nb_live - 1, r, n, now_ns, rv, nullptr, a.comp_sv, ring, out, a.counters, a.sv.run, a.sv.ever, base, lflags, lexp);
+      else final_tile<false, true, true, true>(tile, nb_live - 1, r, n, now_ns, rv, nullptr, a.comp_sv, ring, out, a.counters, a.sv.run, a.sv.ever, base, lflags, lexp);
+      if (stamp) fused_bstamp(a, 10, fused_now());  // (final_tile ends with a block barrier)
     }
   } else if (a.solo) {
     // (tables too big for shared memory, or YDSCHED_FUSED_NOLITE: offsets scanned by the leader of E2)
@@ -697,11 +707,16 @@ __global__ void __launch_bounds__(1024, 1) k_fused_front(FusedArgs a) {
       uint32_t before = 0;  // (thread c) grants of class c in the tiles before this one, from the scanned counts
       if (tid < ncls) {
         const uint32_t* rrow = a.rank_cnt + tid * a.n_rtiles;
-        before = fused_class_grants(a, tid, rrow[tile] - rrow[0], loff[(tid + 1) * a.n_ltiles] - loff[tid * a.n_ltiles]);
+        before = fused_class_grants(a.ct.cls_nelig[tid], rrow[tile] - rrow[0], loff[(tid + 1) * a.n_ltiles] - loff[tid * a.n_ltiles]);
       }
       const uint32_t base = fused_block_sum(before);
       const uint32_t q = tile * 1024 + tid;
-      const uint32_t r = q < n ? fused_select(q, a, loff) : kResEnvNotFound;
+      uint32_t r = kResEnvNotFound;
+      const uint32_t c = q < n ? a.rcls[q] : kNone;  // (kNone: an unknown digest, or one nobody holds)
+      if (c != kNone) {
+        const uint32_t* rrow = a.rank_cnt + c * a.n_rtiles;
+        r = fused_select(c, rrow[q / kRankTile] - rrow[0] + a.rrank[q], a, a.ct.cls_nelig, loff, a.n_ltiles);
+      }
       if (a.packed_out) final_tile<true, true, true>(tile, nb_live - 1, r, n, now_ns, rv, nullptr, a.comp_sv, ring, out, a.counters, a.sv.run, a.sv.ever, base);
       else final_tile<false, true, true>(tile, nb_live - 1, r, n, now_ns, rv, nullptr, a.comp_sv, ring, out, a.counters, a.sv.run, a.sv.ever, base);
     }

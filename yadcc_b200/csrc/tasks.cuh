@@ -142,13 +142,15 @@ __global__ void __launch_bounds__(1024) k_final_write(const uint32_t* __restrict
 // FIFO ordinal of the grant}, see yd_grant8 in ydsched.h.
 // kPos: r is already a registry position (else an index into comp_sv).  kBase: the caller knows the grants of the tiles
 // before this one (`base`; the fused solo kernel derives it from its per-class counts): no look-back, `look` is unused.
-template <bool kPacked, bool kPos = false, bool kBase = false>
+// kLease: the caller has read the request's lease fields already (`lflags`, `lexp`: ReqView::lease), so that their load
+// overlaps its own; else they are read here, once the grant is known.
+template <bool kPacked, bool kPos = false, bool kBase = false, bool kLease = false>
 __device__ __forceinline__ void final_tile(uint32_t vb, uint32_t last_vb, uint32_t r, uint32_t n, long long now_ns,
                                            const ReqView& reqs, unsigned long long* __restrict__ look,
                                            const uint32_t* __restrict__ comp_sv, const TaskRing& ring,
                                            void* __restrict__ out, Counters* __restrict__ counters,
                                            uint32_t* __restrict__ run, unsigned long long* __restrict__ ever,
-                                           unsigned long long base = 0) {
+                                           unsigned long long base = 0, uint32_t lflags = 0, long long lexp = 0) {
   __shared__ uint32_t warp_cnt[32];
   __shared__ unsigned long long s_excl;
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -158,12 +160,26 @@ __device__ __forceinline__ void final_tile(uint32_t vb, uint32_t last_vb, uint32
   const uint32_t bal = __ballot_sync(0xffffffffu, granted);
   if (lane == 0) warp_cnt[warp] = __popc(bal);
   __syncthreads();
-  if (warp == 0) {
-    const uint32_t mine = __reduce_add_sync(0xffffffffu, warp_cnt[lane]);
+  // every warp scans the 32 warp counts itself: its grants in the lower warps, and the tile's
+  uint32_t wpre = warp_cnt[lane];
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const uint32_t y = __shfl_up_sync(0xffffffffu, wpre, d);
+    if (lane >= d) wpre += y;
+  }
+  const uint32_t mine = __shfl_sync(0xffffffffu, wpre, 31);
+  wpre = __shfl_sync(0xffffffffu, wpre, (warp + 31) & 31);
+  if (warp == 0) wpre = 0;
+  if (kBase) {  // the caller knows the tiles before this one: no look-back, no second barrier
+    if (warp == 0 && lane == 0 && vb == last_vb) {  // the last block knows the batch's total
+      counters->granted = base + mine;
+      counters->alive += base + mine;
+    }
+  } else if (warp == 0) {
     volatile unsigned long long* vl = look;
-    if (!kBase && lane == 0) { __threadfence(); vl[vb] = (1ull << 62) | mine; }
-    unsigned long long excl = kBase ? base : 0ull;
-    int at = kBase ? -1 : (int)vb - 1;
+    if (lane == 0) { __threadfence(); vl[vb] = (1ull << 62) | mine; }
+    unsigned long long excl = 0ull;
+    int at = (int)vb - 1;
     while (at >= 0) {
       const int idx = at - (int)lane;
       unsigned long long v;
@@ -187,10 +203,8 @@ __device__ __forceinline__ void final_tile(uint32_t vb, uint32_t last_vb, uint32
       at -= 32;
     }
     if (lane == 0) {
-      if (!kBase) {
-        __threadfence();
-        vl[vb] = (2ull << 62) | (excl + mine);
-      }
+      __threadfence();
+      vl[vb] = (2ull << 62) | (excl + mine);
       s_excl = excl;
       if (vb == last_vb) {  // the last block knows the batch's total
         counters->granted = excl + mine;
@@ -198,20 +212,18 @@ __device__ __forceinline__ void final_tile(uint32_t vb, uint32_t last_vb, uint32
       }
     }
   }
-  __syncthreads();
+  if (!kBase) __syncthreads();
   if (q < n) {
-    uint32_t before = 0;
-    for (uint32_t w = 0; w < warp; ++w) before += warp_cnt[w];
-    before += __popc(bal & ((1u << lane) - 1));
-    const uint64_t ordinal = s_excl + before;
+    const uint32_t before = wpre + __popc(bal & ((1u << lane) - 1));
+    const uint64_t ordinal = (kBase ? base : s_excl) + before;
     uint32_t status;
     if (granted) {
       status = YD_STATUS_GRANTED;
       const uint64_t id = ring.next + ordinal;
       const uint64_t slot = id & ring.mask;
-      uint32_t rflags;
-      long long expires_in_ns;
-      reqs.lease(q, rflags, expires_in_ns);
+      uint32_t rflags = lflags;
+      long long expires_in_ns = lexp;
+      if (!kLease) reqs.lease(q, rflags, expires_in_ns);
       ring.exp[slot] = now_ns + expires_in_ns;
       ring.srv[slot] = r;
       ring.flags[slot] = kTaskAlive | ((rflags & YD_REQ_FLAG_PREFETCH) ? kTaskPrefetch : 0u);

@@ -187,6 +187,7 @@ struct yd_sched {
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr, ev_h2d = nullptr, ev_fin = nullptr;
   uint32_t cls_bound = 16;  // classes the per-class grids are sized for; grows on demand (<= yd::kMaxClasses)
   DevBuf d_list, d_list_bal, d_rcls, d_rrank, d_rank_cnt, d_rq, d_rself;
+  DevBuf d_members;  // the fused solo solve's per-tile member lists (classes.cuh: list_member_index)
   // merge solver (solve_merge.cuh): per-slot verdicts and the chunk boundary states
   DevBuf d_slot_pick, d_mst_in, d_mst_out, d_stream_scratch;
   size_t z_merge_off = 0, z_layout_off = 0, z_final_off = 0, z_scan_off = 0;
@@ -663,7 +664,7 @@ void yd_destroy(yd_sched* s) {
                     &s->d_t_flags, &s->d_reqs, &s->d_res, &s->d_out, &s->d_blk, &s->d_row_off, &s->d_row_len,
                     &s->d_codes, &s->d_ids, &s->d_ok, &s->d_counters, &s->d_sv_env_off, &s->d_sv_envs,
                     &s->d_comp_mode, &s->d_sv_emask, &s->d_slot_rec, &s->d_slot_owner, &s->d_sort_k[0], &s->d_sort_k[1], &s->d_sort_v[0],
-                    &s->d_sort_v[1], &s->d_zero, &s->d_list, &s->d_list_bal, &s->d_rcls, &s->d_rrank, &s->d_rank_cnt, &s->d_rq, &s->d_rself,
+                    &s->d_sort_v[1], &s->d_zero, &s->d_list, &s->d_list_bal, &s->d_members, &s->d_rcls, &s->d_rrank, &s->d_rank_cnt, &s->d_rq, &s->d_rself,
                     &s->d_slot_pick, &s->d_mst_in, &s->d_mst_out, &s->d_stream_scratch, &s->d_reqs16, &s->d_out8, &s->d_fused_prof, &s->d_report, &s->d_bloom,
                     &s->d_bloom_keys, &s->d_bloom_out, &s->d_rt_bytes, &s->d_rt_off, &s->d_rt_len, &s->d_rt_ids,
                     &s->d_rt_slots, &s->d_rt_keys, &s->d_rt_out}) {
@@ -928,6 +929,12 @@ void PrepareStreamBuffers(yd_sched* s, uint32_t Nb, size_t slot_b) {
   s->d_zero.ensure(s->z_bytes);
   s->d_list.ensure(slot_b * 8 * 4);
   s->d_list_bal.ensure(size_t(n_tiles) * s->cls_bound * 32 * 4);  // membership ballots: (tile, list, warp)
+  // member lists of the fused solo solve: (tile, list, rank in the tile), for the batches the fused kernel may take --
+  // cls_bound x tiles <= 32768, so 128 MiB at most (allocated here, before the scratch signature is taken: a buffer
+  // that grew on a steady call would bump g_buf_generation and cost the next solve its speculation)
+  if (s->fused_cfg && Nb <= s->fused_max_nb && size_t(s->cls_bound) * n_tiles <= 32768) {
+    s->d_members.ensure(size_t(n_tiles) * s->cls_bound * yd::kListTile * 4);
+  }
   const uint32_t n_rtiles = (Nb + yd::kRankTile - 1) / yd::kRankTile;
   s->d_rcls.ensure(size_t(Nb) * 4); s->d_rrank.ensure(size_t(Nb) * 4); s->d_rq.ensure(size_t(Nb) * 8);
   s->d_rself.ensure(size_t(Nb) * 4);
@@ -1155,6 +1162,7 @@ uint32_t LaunchFused(yd_sched* s, uint32_t N, size_t slot_b, bool capturing, boo
   a.rank_cnt = s->d_rank_cnt.as<uint32_t>();
   a.list_cnt = reinterpret_cast<uint32_t*>(static_cast<char*>(s->d_zero.p) + s->z_listcnt_off);
   a.list_bal = s->d_list_bal.as<uint32_t>();
+  a.members = s->d_members.as<uint32_t>();
   a.list = s->d_list.as<uint2>();
   a.list_cap = (uint32_t)(slot_b * 4);
   a.rq = s->d_rq.as<uint2>();

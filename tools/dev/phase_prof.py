@@ -3,7 +3,8 @@
 
 For every speculative solve (variant 4) it also prints each block's stamps as min / median / max over the blocks: its
 start, each item of phase A by kind (request tile, slot tile, class), the barrier arrival and wait, phase B and its end
--- in us from the first block's start -- and the CUDA-event time of the same solve, whose excess over the kernel's span
+-- in us from the first block's start --, the links of phase B and the servant counters (from the barrier departure
+of the blocks that count them) and the CUDA-event time of the same solve, whose excess over the kernel's span
 (first block's start to the last block's end) is the launch and the drain."""
 import os, sys, tempfile, time
 os.environ["YDSCHED_FUSED_PROF"] = "1"
@@ -65,6 +66,10 @@ def block_table(line, event_us):
             ("B: selection", (tiled[:, 9] - tiled[:, 8]) / 1e3),
             ("B: final_tile", (tiled[:, 10] - tiled[:, 9]) / 1e3),
         ]
+    # the blocks that counted the servants' grants (word 11), from their barrier departure
+    counting = b[b[:, 11] != 0]
+    if len(counting):
+        rows.append((f"B: servant counters, n={len(counting)}", (counting[:, 11] - counting[:, 5]) / 1e3))
     span = (max(b[:, 6].max(), last_end) - t0) / 1e3
     head = (f"    {G} blocks; kernel span {span:.1f} us (first start .. last block done, report and clean-up included), "
             f"event {event_us:.1f} us, launch + drain {event_us - span:.1f} us")

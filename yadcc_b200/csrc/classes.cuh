@@ -415,15 +415,18 @@ __device__ __forceinline__ bool decode_slot(const SlotDecode& d, const TopoView&
 }
 
 // The kept order's decode, materialised once per rebuild: rec[i] = (registry position, running_tasks value) of sorted
-// slot i, or (kNone, 0) for a slot outside its row.
+// slot i, or (kNone, 0) for a slot outside its row; and its inverse, spos[row_off[pos] + k] = i, the sorted position of
+// every slot of a row (the speculative solve counts a servant's grants from it, fused.cuh: fused_servant_counters).
 __global__ void __launch_bounds__(256) k_slot_records(const unsigned long long* __restrict__ m_ptr, SlotDecode d,
-                                                      uint2* __restrict__ rec) {
+                                                      uint2* __restrict__ rec, uint32_t* __restrict__ spos) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (uint32_t)*m_ptr) return;
   const uint32_t orig = d.sorted_orig[i];
   const uint32_t pos = d.slot_owner[orig];
   const uint32_t k = orig - d.row_off[pos];
-  rec[i] = k < d.row_len[pos] ? make_uint2(pos, k) : make_uint2(kNone, 0u);
+  const bool in_row = k < d.row_len[pos];
+  rec[i] = in_row ? make_uint2(pos, k) : make_uint2(kNone, 0u);
+  if (in_row) spos[orig] = i;
 }
 
 // "Slot i belongs to list c" is evaluated ONCE, by the count kernel, as ballots: one 32-bit
@@ -441,9 +444,14 @@ __shared__ uint32_t s_count_bal[kListChunk][32];
 // made: members[(tile * cls_bound + c) * kListTile + j] = the registry position of the j-th member of list c inside slot
 // tile `tile` (j = the member's rank in the tile's list: members of the list in lower warps + in lower lanes of its
 // warp).  A solo solve's components with requests hold one class each, so a slot is in one list at most.
+// The speculative solve's words (list_count_tile_kept) also carry the member's slot index inside the tile above the
+// position: pos | slot << kMemberSlotShift.  The host speculates only while the registry holds fewer than 2^22 servants.
 __device__ __forceinline__ size_t list_member_index(uint32_t tile, uint32_t c, uint32_t cls_bound) {
   return (size_t(tile) * cls_bound + c) * kListTile;
 }
+constexpr uint32_t kMemberSlotShift = 22;
+constexpr uint32_t kMemberPosMask = (1u << kMemberSlotShift) - 1;
+static_assert((1ull << 32 >> kMemberSlotShift) == kListTile, "a member word holds the slot's index inside its tile in its top bits");
 
 // The counts of lists c0 .. c1 in this tile from the chunk's ballots in s_count_bal (warp c - c0 takes list c).
 // `prefix`: each ballot word is then replaced by the list's members in the lower warps (the member lists' offsets).
@@ -519,7 +527,7 @@ __device__ __forceinline__ void list_count_tile(uint32_t tile, uint32_t m, const
 // So: three gathers per slot (run, kept_sv, version) instead of four to five, one test, and the lanes of a warp grouped
 // by list (__match_any_sync) instead of one ballot per class.  s_mv: the classes' min_versions in shared memory, loaded
 // by the block's first call (`facts`).  It writes the member lists (list_member_index), not the ballot words: the
-// speculative solve selects from the member lists alone.
+// speculative solve selects from the member lists alone.  Each word carries the slot's index inside the tile too.
 __device__ __forceinline__ void list_count_tile_kept(uint32_t tile, uint32_t m, uint32_t ncls, const SlotDecode& d,
                                                      const ClassTable& ct, const ServantArrays& sv,
                                                      const uint32_t* __restrict__ kept_sv, uint32_t n_tiles,
@@ -551,7 +559,8 @@ __device__ __forceinline__ void list_count_tile_kept(uint32_t tile, uint32_t m, 
     list_chunk_counts(c0, c1, tile, n_tiles, counts, true);
     __syncthreads();
     if (key != kNone) {
-      members[list_member_index(tile, key, ct.cls_bound) + bal[key - c0][warp] + __popc(peers & ((1u << lane) - 1))] = rec.x;
+      members[list_member_index(tile, key, ct.cls_bound) + bal[key - c0][warp] + __popc(peers & ((1u << lane) - 1))] =
+          rec.x | tid << kMemberSlotShift;
     }
     __syncthreads();  // the ballots have been consumed
   }

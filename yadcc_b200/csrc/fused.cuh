@@ -31,7 +31,9 @@
 //       (list_count_tile_kept); eligible servants per class (servant versions and max_tasks change without a new
 //       topology)
 //   --  barrier
-//   B   P6 as above (the lite selection, closed-form task ids).  The last block resets the barrier words, nothing else.
+//   B   P6 as above (the lite selection, closed-form task ids), without the per-grant running_tasks / ever atomics:
+//       each servant's grants are counted once, by one warp, in blocks without a request tile
+//       (fused_servant_counters).  The last block resets the barrier words, nothing else.
 //
 // A request MISSES when its digest is held by a component but its class is not in the table, or when its IP is that of
 // a servant of its component: flag kFlagSpecMiss, nothing is decided, the last block clears the scratch (the kept table
@@ -131,6 +133,7 @@ struct FusedArgs {
   uint32_t spec;              // solo, speculative: the class table kept from the last solo solve, one grid barrier
   uint4* kept_env;            // [n_envs] the kept class table per digest (classes.cuh: kept_class) ...
   uint32_t* kept_sv;          // [n_servants] ... and per servant (list_count_tile_kept); both written with the table
+  const uint32_t* slot_spos;  // the kept order's sorted position of every row slot (k_slot_records)
   unsigned long long* prof;  // debug (YDSCHED_FUSED_PROF): %globaltimer stamps (kProfHead / kProfBlockWords), else null
 };
 
@@ -138,7 +141,8 @@ struct FusedArgs {
 // block b, prof[kProfHead + b * kProfBlockWords + k]: k = 0 start, 1..3 end of its first three items of phase A, 4
 // barrier arrival, 5 departure, 6 end of phase B; word 7 = the kinds of those items (4 bits each, FusedItem) | the
 // number of items << 16; then, for the block's first request tile of phase B, 8 end of the table build (list offsets,
-// request prefixes, base), 9 end of the selection, 10 end of final_tile; word 11 is unused.
+// request prefixes, base), 9 end of the selection, 10 end of final_tile; word 11 = end of the servant counters
+// (fused_servant_counters), in the blocks that count them.
 constexpr uint32_t kProfHead = 16;
 constexpr uint32_t kProfBlockWords = 12;
 constexpr uint32_t kProfMaxItems = 3;
@@ -365,7 +369,7 @@ __device__ __forceinline__ uint32_t fused_select(uint32_t c, uint32_t rank, cons
     const uint32_t mid = (lo + hi) >> 1;
     if (row[mid] <= target) lo = mid; else hi = mid;
   }
-  return a.members[list_member_index(lo, c, a.ct.cls_bound) + (target - row[lo])];
+  return a.members[list_member_index(lo, c, a.ct.cls_bound) + (target - row[lo])] & kMemberPosMask;
 }
 
 // Task ids of a solo solve in closed form.  The selection above grants the class-c request with class rank k exactly
@@ -375,6 +379,106 @@ __device__ __forceinline__ uint32_t fused_select(uint32_t c, uint32_t rank, cons
 __device__ __forceinline__ uint32_t fused_class_grants(uint32_t nelig, uint32_t before, uint32_t len) {
   return nelig != 0 ? min(before, len) : 0u;
 }
+
+// Speculative solve: ++running_tasks and ++ever_assigned_tasks of every grant, counted per servant instead of two
+// atomics per grant in final_tile (on a few hundred lines, which L2 applies one after the other).  The grants of class c
+// are the first L'_c = nelig_c ? min(R_c, L_c) : 0 members of its list (R_c requests, L_c members: fused_class_grants),
+// and the list is in sorted-slot order.  So servant s, of class c = kept_sv[s] and a version high enough (the test of
+// list_count_tile_kept), receives one grant per slot r in [run[s], row_len[s]) whose sorted position (slot_spos) is at
+// most that of the list's member at rank L'_c - 1, whose slot the member word names.  One warp per class finds that
+// bound, then one warp per servant counts its slots below it and writes run[s] and ever[s] with plain stores: after the
+// barrier nothing else reads or writes them.  The servants' facts and the sorted positions of their first 64 free slots
+// do not depend on the bounds: they are loaded first, two servants per warp, so that their two round trips overlap the
+// two of the bounds (the class rows, then one member word).  `own` / `n_own`: this block's index among the blocks that
+// share the servants, and their number.
+__device__ __forceinline__ void fused_servant_counters(const FusedArgs& a, uint32_t ncls, uint32_t nb_live, uint32_t own,
+                                                       uint32_t n_own) {
+  __shared__ uint32_t s_end[kMaxClasses];  // class c grants its list's members at sorted positions below s_end[c]
+  __shared__ uint32_t s_mv[kMaxClasses];
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const uint32_t W = n_own * 32, gw = own * 32 + warp;  // this warp's servants: gw + j * W
+  uint32_t sc[2], sver[2], srun[2], soff[2], slen[2], sp[2][2];
+  unsigned long long sever[2];
+  auto fetch = [&](uint32_t s0) {
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const uint32_t s = s0 + j * W;
+      const bool in = s < a.n_servants;
+      sc[j] = in ? a.kept_sv[s] : kNone;
+      sver[j] = in ? (uint32_t)a.sv.version[s] : 0u;
+      srun[j] = in ? a.sv.run[s] : 0u;
+      soff[j] = in ? a.dec.row_off[s] : 0u;
+      slen[j] = in ? a.dec.row_len[s] : 0u;
+      sever[j] = in ? a.sv.ever[s] : 0ull;
+    }
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const uint32_t r = srun[j] + h * 32 + lane;
+        sp[j][h] = sc[j] < ncls && r < slen[j] ? a.slot_spos[soff[j] + r] : kNone;
+      }
+    }
+  };
+  fetch(gw);
+  for (uint32_t c = warp; c < ncls; c += 32) {
+    const uint32_t* rrow = a.rank_cnt + c * a.n_rtiles;
+    const uint32_t* lrow = a.list_cnt + c * a.n_ltiles;
+    const uint32_t nelig = a.ct.cls_nelig[c], mv = a.ct.cls_mv[c];
+    uint32_t R = 0, L = 0;
+#pragma unroll 4
+    for (uint32_t t = lane; t < nb_live; t += 32) R += rrow[t];
+#pragma unroll 4
+    for (uint32_t t = lane; t < a.n_ltiles; t += 32) L += lrow[t];
+    R = __reduce_add_sync(0xffffffffu, R);
+    L = __reduce_add_sync(0xffffffffu, L);
+    const uint32_t take = fused_class_grants(nelig, R, L);
+    uint32_t end = 0;
+    if (take) {  // the slot tile of the member at rank take - 1 (the first whose inclusive prefix exceeds it) and its word
+      const uint32_t target = take - 1;
+      for (uint32_t t0 = 0, before = 0; t0 < a.n_ltiles; t0 += 32) {
+        const uint32_t t = t0 + lane, v = t < a.n_ltiles ? lrow[t] : 0u;
+        uint32_t x = v;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+          const uint32_t y = __shfl_up_sync(0xffffffffu, x, d);
+          if (lane >= d) x += y;
+        }
+        const uint32_t past = __ballot_sync(0xffffffffu, before + x > target);
+        if (past) {
+          const uint32_t l = __ffs(past) - 1;
+          const uint32_t pre = __shfl_sync(0xffffffffu, before + x - v, l);
+          const uint32_t w = a.members[list_member_index(t0 + l, c, a.ct.cls_bound) + (target - pre)];
+          end = (t0 + l) * kListTile + (w >> kMemberSlotShift) + 1;
+          break;
+        }
+        before += __shfl_sync(0xffffffffu, x, 31);
+      }
+    }
+    if (lane == 0) { s_end[c] = end; s_mv[c] = mv; }
+  }
+  __syncthreads();
+  for (uint32_t s0 = gw; s0 < a.n_servants; s0 += 2 * W) {
+    if (s0 != gw) fetch(s0);
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const uint32_t s = s0 + j * W, c = sc[j];
+      if (c >= ncls || sver[j] < s_mv[c] || s_end[c] == 0) continue;  // (the same for the whole warp; kNone beyond S)
+      const uint32_t end = s_end[c];
+      uint32_t k = (sp[j][0] < end ? 1u : 0u) + (sp[j][1] < end ? 1u : 0u);
+      for (uint32_t r = srun[j] + 64 + lane; r < slen[j]; r += 32) k += a.slot_spos[soff[j] + r] < end ? 1u : 0u;
+      k = __reduce_add_sync(0xffffffffu, k);
+      if (lane == 0 && k) {
+        a.sv.run[s] = srun[j] + k;
+        a.sv.ever[s] = sever[j] + k;
+      }
+    }
+  }
+}
+
+// Blocks that take the servant counters of a speculative solve: those without a request tile when there are at least
+// this many, else every block (after its request tiles).
+constexpr uint32_t kCounterMinBlocks = 16;
 
 // Request q = tile * 1024 + thread (a block of 1024 threads): its digest id, min_version and requestor IP; false beyond
 // the queue's end.  A zero-copy solve first copies the tile from the caller's page-locked array to HBM (every later read
@@ -453,6 +557,12 @@ __global__ void __launch_bounds__(1024, 1) k_fused_front(FusedArgs a) {
     if (a.spec) {
       fused_prefetch(a.kept_env, size_t(a.t.n_envs) * sizeof(uint4));
       fused_prefetch(a.t.ip_comp_mask, size_t(a.t.n_ips) * 8);
+      // (fused_servant_counters)
+      fused_prefetch(a.kept_sv, S4);
+      fused_prefetch(a.sv.ever, S4 * 2);
+      fused_prefetch(a.dec.row_off, S4);
+      fused_prefetch(a.dec.row_len, S4);
+      fused_prefetch(a.slot_spos, size_t(m) * 4);
     }
     fused_prefetch(a.dec.rec, size_t(m) * 8);
     fused_prefetch(a.sv.run, S4);
@@ -690,9 +800,24 @@ __global__ void __launch_bounds__(1024, 1) k_fused_front(FusedArgs a) {
         __syncthreads();  // (every selection of the tile is done)
         fused_bstamp(a, 9, fused_now());
       }
-      if (a.packed_out) final_tile<true, true, true, true>(tile, nb_live - 1, r, n, now_ns, rv, nullptr, a.comp_sv, ring, out, a.counters, a.sv.run, a.sv.ever, base, lflags, lexp);
-      else final_tile<false, true, true, true>(tile, nb_live - 1, r, n, now_ns, rv, nullptr, a.comp_sv, ring, out, a.counters, a.sv.run, a.sv.ever, base, lflags, lexp);
+      if (a.spec) {  // (the servant counters are counted below)
+        if (a.packed_out) final_tile<true, true, true, true, false>(tile, nb_live - 1, r, n, now_ns, rv, nullptr, a.comp_sv, ring, out, a.counters, a.sv.run, a.sv.ever, base, lflags, lexp);
+        else final_tile<false, true, true, true, false>(tile, nb_live - 1, r, n, now_ns, rv, nullptr, a.comp_sv, ring, out, a.counters, a.sv.run, a.sv.ever, base, lflags, lexp);
+      } else {
+        if (a.packed_out) final_tile<true, true, true, true>(tile, nb_live - 1, r, n, now_ns, rv, nullptr, a.comp_sv, ring, out, a.counters, a.sv.run, a.sv.ever, base, lflags, lexp);
+        else final_tile<false, true, true, true>(tile, nb_live - 1, r, n, now_ns, rv, nullptr, a.comp_sv, ring, out, a.counters, a.sv.run, a.sv.ever, base, lflags, lexp);
+      }
       if (stamp) fused_bstamp(a, 10, fused_now());  // (final_tile ends with a block barrier)
+    }
+    if (a.spec) {
+      const bool idle = G >= nb_live + kCounterMinBlocks;  // enough blocks without a request tile
+      if (!idle || blockIdx.x >= nb_live) {
+        fused_servant_counters(a, ncls, nb_live, idle ? blockIdx.x - nb_live : blockIdx.x, idle ? G - nb_live : G);
+        if (a.prof) {
+          __syncthreads();
+          fused_bstamp(a, 11, fused_now());
+        }
+      }
     }
   } else if (a.solo) {
     // (tables too big for shared memory, or YDSCHED_FUSED_NOLITE: offsets scanned by the leader of E2)

@@ -143,8 +143,9 @@ __global__ void __launch_bounds__(1024) k_final_write(const uint32_t* __restrict
 // kPos: r is already a registry position (else an index into comp_sv).  kBase: the caller knows the grants of the tiles
 // before this one (`base`; the fused solo kernel derives it from its per-class counts): no look-back, `look` is unused.
 // kLease: the caller has read the request's lease fields already (`lflags`, `lexp`: ReqView::lease), so that their load
-// overlaps its own; else they are read here, once the grant is known.
-template <bool kPacked, bool kPos = false, bool kBase = false, bool kLease = false>
+// overlaps its own; else they are read here, once the grant is known.  kCount: ++running_tasks and ++ever of the
+// granted servant, one atomic each per grant (the speculative solo solve counts them per servant instead, fused.cuh).
+template <bool kPacked, bool kPos = false, bool kBase = false, bool kLease = false, bool kCount = true>
 __device__ __forceinline__ void final_tile(uint32_t vb, uint32_t last_vb, uint32_t r, uint32_t n, long long now_ns,
                                            const ReqView& reqs, unsigned long long* __restrict__ look,
                                            const uint32_t* __restrict__ comp_sv, const TaskRing& ring,
@@ -227,8 +228,10 @@ __device__ __forceinline__ void final_tile(uint32_t vb, uint32_t last_vb, uint32
       ring.exp[slot] = now_ns + expires_in_ns;
       ring.srv[slot] = r;
       ring.flags[slot] = kTaskAlive | ((rflags & YD_REQ_FLAG_PREFETCH) ? kTaskPrefetch : 0u);
-      atomicAdd(&run[r], 1u);  // ++running_tasks, ++ever_assigned_tasks (cc:123-124)
-      atomicAdd(&ever[r], 1ull);
+      if (kCount) {
+        atomicAdd(&run[r], 1u);  // ++running_tasks, ++ever_assigned_tasks (cc:123-124)
+        atomicAdd(&ever[r], 1ull);
+      }
     } else {
       status = (r == kResTimeout) ? YD_STATUS_TIMEOUT : YD_STATUS_ENVIRONMENT_NOT_FOUND;
       r = YD_NO_SERVANT;

@@ -175,7 +175,7 @@ struct yd_sched {
   PinBuf h_topo;
 
   // slot-stream solver state
-  DevBuf d_sv_env_off, d_sv_envs, d_comp_mode, d_sv_emask, d_slot_rec;
+  DevBuf d_sv_env_off, d_sv_envs, d_comp_mode, d_sv_emask, d_slot_rec, d_slot_spos;
   bool emask_ok = false;  // every component holds <= 64 digests: d_sv_emask is valid
   DevBuf d_slot_owner, d_sort_k[2], d_sort_v[2];
   // one zero-filled scratch region per solve: radix histograms (one per pass), the class
@@ -663,7 +663,7 @@ void yd_destroy(yd_sched* s) {
                     &s->d_t_exp, &s->d_t_srv,
                     &s->d_t_flags, &s->d_reqs, &s->d_res, &s->d_out, &s->d_blk, &s->d_row_off, &s->d_row_len,
                     &s->d_codes, &s->d_ids, &s->d_ok, &s->d_counters, &s->d_sv_env_off, &s->d_sv_envs,
-                    &s->d_comp_mode, &s->d_sv_emask, &s->d_slot_rec, &s->d_slot_owner, &s->d_sort_k[0], &s->d_sort_k[1], &s->d_sort_v[0],
+                    &s->d_comp_mode, &s->d_sv_emask, &s->d_slot_rec, &s->d_slot_spos, &s->d_slot_owner, &s->d_sort_k[0], &s->d_sort_k[1], &s->d_sort_v[0],
                     &s->d_sort_v[1], &s->d_zero, &s->d_list, &s->d_list_bal, &s->d_members, &s->d_rcls, &s->d_rrank, &s->d_rank_cnt, &s->d_rq, &s->d_rself,
                     &s->d_slot_pick, &s->d_mst_in, &s->d_mst_out, &s->d_stream_scratch, &s->d_reqs16, &s->d_out8, &s->d_fused_prof, &s->d_report, &s->d_bloom,
                     &s->d_bloom_keys, &s->d_bloom_out, &s->d_rt_bytes, &s->d_rt_off, &s->d_rt_len, &s->d_rt_ids,
@@ -905,6 +905,7 @@ void PrepareStreamBuffers(yd_sched* s, uint32_t Nb, size_t slot_b) {
   const size_t ksz = s->wide ? 8 : 4;
   for (int b = 0; b < 2; ++b) { s->d_sort_k[b].ensure(slot_b * ksz); s->d_sort_v[b].ensure(slot_b * 4); }
   s->d_slot_rec.ensure(slot_b * 8);
+  s->d_slot_spos.ensure(slot_b * 4);
   s->sort_nb = (uint32_t)((slot_b + yd::kRsTile - 1) / yd::kRsTile);
   const int passes = s->wide ? 9 : 4;
   size_t off = 0;
@@ -989,7 +990,8 @@ uint32_t RebuildSlotOrder(yd_sched* s, size_t slot_b) {
     yd::SlotDecode dec{s->d_sort_v[0].as<uint32_t>(), s->d_slot_owner.as<uint32_t>(), s->d_row_off.as<uint32_t>(),
                        s->d_row_len.as<uint32_t>(), s->d_run.as<uint32_t>(), 1u, nullptr};
     yd::k_slot_records<<<(unsigned)((slot_b + 255) / 256), 256, 0, st>>>(&s->d_counters.as<Counters>()->slots, dec,
-                                                                          s->d_slot_rec.as<uint2>());
+                                                                          s->d_slot_rec.as<uint2>(),
+                                                                          s->d_slot_spos.as<uint32_t>());
     l += 1;
   }
   YD_CUDA_CHECK(cudaGetLastError());
@@ -1187,6 +1189,7 @@ uint32_t LaunchFused(yd_sched* s, uint32_t N, size_t slot_b, bool capturing, boo
   a.spec = spec ? 1u : 0u;
   a.kept_env = s->d_kept_env.as<uint4>();
   a.kept_sv = s->d_kept_sv.as<uint32_t>();
+  a.slot_spos = s->d_slot_spos.as<uint32_t>();
   yd::k_fused_front<<<grid, 1024, dyn, st>>>(a);
   s->last_fused = a;
   s->last_fused_grid = grid;
@@ -1546,11 +1549,13 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
       if (solver == 2) PrepareStreamBuffers(s, Nb, slot_b);  // (fixes the scratch layout the signature describes)
       sig_now = yd_sched::CleanSig{g_buf_generation, s->z_cls_off, s->z_bytes, s->res_words, s->d_zero.p, s->d_res.p};
       // speculative (fused.cuh): the kept class table is the one these buffers, this topology and this class bound
-      // had; every block holds at most two request tiles (their classes and ranks stay in registers) and the lists'
-      // offsets fit in shared memory (the selection without leader scans)
+      // had; every block holds at most two request tiles (their classes and ranks stay in registers), the lists'
+      // offsets fit in shared memory (the selection without leader scans), and registry positions fit the member words
+      // below the slot's index in its tile (classes.cuh: kMemberSlotShift)
       const size_t lcells = size_t(s->cls_bound) * ((slot_b + yd::kListTile - 1) / yd::kListTile + 1) + 1;
       if (s->kept_valid && s->kept_sig == yd_sched::KeptSig{sig_now, s->topo_gen, s->cls_bound} && s->fused_lite &&
-          lcells <= kFusedLoffCacheWords && (Nb + yd::kRankTile - 1) / yd::kRankTile <= 2 * s->fused_grid) {
+          lcells <= kFusedLoffCacheWords && (Nb + yd::kRankTile - 1) / yd::kRankTile <= 2 * s->fused_grid &&
+          S <= yd::kMemberPosMask) {
         variant = 4;  // the graph is the kernel alone
       } else if (s->clean_valid && s->clean_sig == sig_now) {
         variant = 3;  // no memset nodes: the graph is the kernel alone

@@ -4,9 +4,9 @@ with one load.  The cases sit at the index's edges: a class that owns every slot
 start, end or skip at tile boundaries, a last slot tile that is only partly filled, dead slots between live ones
 (servants that are partly busy, below the batch's min_version or with max_tasks = 0), and more classes than one chunk of
 lists (kListChunk) holds.  Every stream is replayed through the CUDA backend -- plain, packed and staged calls -- and
-compared with the CPU checker; the YDSCHED_DEBUG solve lines show that it reached the speculative solve (variant 4), the
-solo solve that keeps its class table (variants 2 / 3) and, with YDSCHED_FUSED_NOLITE, the selection from the leader's
-scanned offsets."""
+compared with the CPU checker; the YDSCHED_DEBUG solve lines show that it reached the speculative solve (variant 4) and
+the solo solve that keeps its class table (variants 2 / 3).  Each case also runs next to a wide table whose list offsets
+do not fit in shared memory, where the solo solve selects from the leader's scanned offsets."""
 import numpy as np
 import pytest
 
@@ -48,8 +48,20 @@ def _case(name):
     raise ValueError(name)
 
 
-def _stream(d, name, seed=3):
-    servants, n_digests, n, asked, free = _case(name)
+# 130 more digests on 520 servants of capacity 64, each digest asked for twice per batch: the class bound grows to 256
+# and the static slot bound passes 33 800 slots (64 slot tiles), so the list offsets, 256 x 65 + 1 words, no longer fit
+# in shared memory (16 384 words)
+WIDE_DIGESTS, WIDE_SERVANTS, WIDE_ASKS = 130, 520, 2
+
+
+def _stream(d, name, wide, seed=3):
+    servants, n_digests, n_case, asked, free = _case(name)
+    wide_asks = []
+    if wide:
+        servants = servants + [(n_digests + i % WIDE_DIGESTS, 10, 64) for i in range(WIDE_SERVANTS)]
+        wide_asks = list(range(n_digests, n_digests + WIDE_DIGESTS)) * WIDE_ASKS
+        n_digests += WIDE_DIGESTS
+    n = n_case + len(wide_asks)
     dg = _digests(n_digests)
     ev = [("hb", 0.0, _servant(i, [dg[k]], v, mt), 100.0) for i, (k, v, mt) in enumerate(servants)]
     env = np.asarray([d.intern_env(x) for x in dg], dtype=np.uint32)
@@ -57,7 +69,9 @@ def _stream(d, name, seed=3):
     rng = np.random.default_rng(seed)
     now = 0.001
     for _ in range(7):  # one class set: the first solves keep the class table, the later ones speculate
-        e = env[np.asarray(asked)[rng.integers(0, len(asked), n)]]
+        e = env[np.asarray(asked)[rng.integers(0, len(asked), n_case)]]
+        if wide:
+            e = rng.permutation(np.concatenate([e, env[wide_asks]]))
         ips = outside[rng.integers(0, len(outside), n)]
         ev.append(("wait", now, S._requests(d, e, ips, np.full(n, 8, np.uint32), expires_in_s=15.0,
                                             prefetch=rng.random(n) < 0.2)))
@@ -68,17 +82,16 @@ def _stream(d, name, seed=3):
     return S.Stream(f"members-{name}", ev), n
 
 
-@pytest.mark.parametrize("nolite", [False, True], ids=["lite", "nolite"])
+@pytest.mark.parametrize("selection", ["lite", "leader-scan"])
 @pytest.mark.parametrize("mode", ["plain", "packed", "staged"])
 @pytest.mark.parametrize("case", ["full-tile", "boundaries", "dead-slots", "many-classes"])
-def test_member_lists_equal_oracle(make_dispatcher, monkeypatch, capfd, case, mode, nolite):
+def test_member_lists_equal_oracle(make_dispatcher, monkeypatch, capfd, case, mode, selection):
     monkeypatch.setenv("YDSCHED_DEBUG", "1")
-    if nolite:
-        monkeypatch.setenv("YDSCHED_FUSED_NOLITE", "1")
+    wide = selection == "leader-scan"
     traces = {}
     for kind in ("cuda", "port"):
         d = make_dispatcher(kind)
-        stream, n = _stream(d, case)
+        stream, n = _stream(d, case, wide)
         cuda = kind == "cuda"
         traces[kind] = S.Replayer(d, pinned=cuda, packed=(mode == "packed" and cuda),
                                   staged=(mode == "staged" and cuda)).run(stream)
@@ -87,7 +100,8 @@ def test_member_lists_equal_oracle(make_dispatcher, monkeypatch, capfd, case, mo
     lines = [x for x in solves(capfd.readouterr().err) if x["n"] == n]
     variants = [x["variant"] for x in lines]
     assert set(variants) & {2, 3}, variants  # the solo solve that keeps the class table ...
-    if nolite:
+    if wide:
         assert 4 not in variants, variants  # (no speculation without the block-local tables)
+        assert all(x["cls_bound"] * (x["slot_b"] // 1024 + 1) + 1 > 16384 for x in lines if x["variant"] in (2, 3)), lines
     else:
         assert any(x["variant"] == 4 and x["spec"] == 1 for x in lines), variants  # ... and the speculative one

@@ -128,8 +128,8 @@ struct FusedArgs {
   void* out;
   Counters* counters;
   uint32_t n_servants;
-  uint32_t loff_cache_words;  // dynamic shared memory of the launch, in words
-  uint32_t lite;              // solo: no leader scans -- every block derives the offsets it needs from the raw counts
+  uint32_t loff_cache_words;  // solo: dynamic shared memory of the launch, in words; not 0: no leader scans -- every block
+                              // derives the list offsets it needs from the raw counts (the host sizes it when they fit)
   uint32_t spec;              // solo, speculative: the class table kept from the last solo solve, one grid barrier
   uint4* kept_env;            // [n_envs] the kept class table per digest (classes.cuh: kept_class) ...
   uint32_t* kept_sv;          // [n_servants] ... and per servant (list_count_tile_kept); both written with the table
@@ -253,8 +253,8 @@ __device__ __forceinline__ uint32_t fused_block_sum(uint32_t v) {
 }
 
 // The result record for the host (threads 0..8 of one block): the class table's meta words and the grant count, as
-// posted writes into mapped host memory -- or, `report_dev`, into HBM for a copy node to fetch.  The host reads it after
-// the stream has drained, so no ordering is needed among the writes.
+// posted writes into mapped host memory.  The host reads it after the stream has drained, so no ordering is needed
+// among the writes.
 __device__ __forceinline__ void fused_report(const FusedArgs& a, unsigned long long seq, unsigned long long granted,
                                              unsigned long long fp = 0) {
   FusedHostIO* h = a.hio;
@@ -576,7 +576,7 @@ __global__ void __launch_bounds__(1024, 1) k_fused_front(FusedArgs a) {
   }
   const char* zc_in = reinterpret_cast<const char*>(s_zc_in);
   uint32_t ncls, nlists;
-  bool lite;
+  const bool lite = a.solo && a.loff_cache_words != 0;  // (the host speculates only when it holds)
   // speculative: class | in-tile rank << 16 of this thread's request in the block's first / second request tile
   uint32_t spec_cr0 = 0xffffu, spec_cr1 = 0xffffu;
   if (a.spec) {
@@ -620,7 +620,6 @@ __global__ void __launch_bounds__(1024, 1) k_fused_front(FusedArgs a) {
     for (uint32_t i = blockIdx.x * 1024 + tid; i < nlists * tail; i += G * 1024) a.list_cnt[(i / tail) * a.n_ltiles + lt_live + i % tail] = 0;
     // (meta[1] is for the report; the barrier tells the blocks)
     if (__any_sync(0xffffffffu, miss) && (tid & 31) == 0) atomicExch(&a.ct.meta[1], kFlagSpecMiss);
-    lite = true;  // (the host speculates only when the lists' offsets fit in shared memory)
     fused_stamp(a, 1);
     fused_bstamp(a, 4, fused_now());
     const bool missed = fused_barrier_any(a.bar, 1, miss);
@@ -683,7 +682,6 @@ __global__ void __launch_bounds__(1024, 1) k_fused_front(FusedArgs a) {
 
   fused_stamp(a, 3);
   // ---- E2: both count matrices -> offsets (class-major, tile-minor, + the end cell) -------------------------------
-  lite = a.solo && a.lite && nlists * (a.n_ltiles + 1) <= a.loff_cache_words;  // (the same in every block)
   if (lite) {
     fused_barrier(a.bar, 2);  // the counts stay raw: each block derives what it needs below
   } else if (fused_arrive(a.bar, 2)) {
@@ -715,7 +713,7 @@ __global__ void __launch_bounds__(1024, 1) k_fused_front(FusedArgs a) {
   TaskRing ring = a.ring;
   ring.next = s_dyn.ring_next;
   void* const out = s_zc_out ? reinterpret_cast<void*>(s_zc_out) : a.out;
-  if (a.solo && lite) {
+  if (lite) {
     // every component with requests is data-parallel: no lists, each request's member is picked from the per-tile member
     // lists; the tables the selection searches are built here, per block, from the raw (class, tile) counts.  Every load
     // of those tables, the request's class and rank (not speculative) and its lease fields (final_tile) are issued before
@@ -820,14 +818,8 @@ __global__ void __launch_bounds__(1024, 1) k_fused_front(FusedArgs a) {
       }
     }
   } else if (a.solo) {
-    // (tables too big for shared memory, or YDSCHED_FUSED_NOLITE: offsets scanned by the leader of E2)
-    const uint32_t cells = nlists * a.n_ltiles + 1;
+    // (offsets too big for shared memory: scanned by the leader of E2)
     const uint32_t* loff = a.list_cnt;
-    if (cells <= a.loff_cache_words) {
-      for (uint32_t i = tid; i < cells; i += 1024) s_loff[i] = a.list_cnt[i];
-      __syncthreads();
-      loff = s_loff;
-    }
     for (uint32_t tile = blockIdx.x; tile < nb_live; tile += G) {
       uint32_t before = 0;  // (thread c) grants of class c in the tiles before this one, from the scanned counts
       if (tid < ncls) {

@@ -41,7 +41,6 @@ struct StreamArgs {
   const uint32_t* comp_mode;  // [C] 0 = this kernel, 1 = handled by the parallel path, 2 = merge solver ...
   const uint32_t* viol;       // [C] ... unless it handed the component back (solve_merge.cuh)
   Counters* counters;         // pad[0..3]: speculation steps, lanes committed by them, exact walks, walk windows
-  uint32_t debug;             // test switches: bit 0 producers never pre-answer, bit 1 no speculation
 };
 
 struct StreamShared {
@@ -77,7 +76,7 @@ __device__ __forceinline__ void produce_tile_stream(const StreamArgs& a, StreamS
         const uint32_t slot = cls_find(a.ct.keys, ((unsigned long long)env << 32) | mv);
         cls = slot != kNone ? a.ct.slot_cls[slot] : kNone;
         if (cls != kNone) {
-          const uint8_t f = (a.debug & 1u) ? (uint8_t)0 : sh.fail[cls];
+          const uint8_t f = sh.fail[cls];
           if (f) a.res[q] = stream_fail_res(f);
           else mine = true;
         }
@@ -210,7 +209,7 @@ __global__ void __launch_bounds__((kStreamProducers + 1) * 32, 1) k_solve_stream
   // pure overhead; after a short commit the next `cooldown` requests go straight to the
   // exact walk.
   const uint32_t lt_mask = (1u << lane) - 1;
-  uint32_t cooldown = (a.debug & 2u) ? 0x7fffffffu : 0u;
+  uint32_t cooldown = 0;
   unsigned long long st_steps = 0, st_lanes = 0, st_walks = 0, st_windows = 0;
   for (uint32_t t = 0; t < n_tiles; ++t) {
     const uint32_t buf = t & 1;

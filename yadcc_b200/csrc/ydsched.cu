@@ -133,6 +133,85 @@ struct RunningRec {
   std::string servant_location, task_digest;
 };
 
+// The sequence of a slot-stream solve (EnqueueSolve); the YDSCHED_DEBUG line prints the number.
+enum SolveVariant : uint32_t {
+  kPipeline = 0,   // the kernel-by-kernel pipeline
+  kFused = 1,      // fused front (fused.cuh) + coupled solvers + final
+  kSolo = 2,       // the fused front alone: it writes the grants too
+  kSoloClean = 3,  // the same on a clean scratch (no memset nodes)
+  kSoloSpec = 4,   // solo and speculative on the kept class table (no memsets)
+};
+constexpr bool IsSolo(SolveVariant v) { return v == kSolo || v == kSoloClean || v == kSoloSpec; }
+
+// One attempt of a solve.  A stand-down escalates the merge rounds or the solver here, never in the configured values.
+struct SolvePlan {
+  SolveVariant variant;
+  uint32_t solver;        // 1 row scan, 2 slot streams
+  uint32_t merge_rounds;  // (a graph key: a settled merge needs fewer)
+  uint32_t force_stream;  // ClassTable::force_stream
+};
+
+// The solo kernel re-initialises the scratch it dirtied (class-table keys, zeroed region) before it ends; while this
+// signature matches the current buffers and layout the next solo solve needs no memset nodes either.
+struct CleanSig { unsigned long long gen = ~0ull; size_t z_cls_off = 0, z_bytes = 0, res_words = 0; const void* zero = nullptr; const void* res = nullptr;
+  bool operator==(const CleanSig& o) const { return gen == o.gen && z_cls_off == o.z_cls_off && z_bytes == o.z_bytes && res_words == o.res_words && zero == o.zero && res == o.res; } };
+// A kept class table is valid for the buffers, the topology and the class bound it was built with.
+struct KeptSig { CleanSig clean; unsigned long long topo_gen = 0; uint32_t cls_bound = 0;
+  bool operator==(const KeptSig& o) const { return clean == o.clean && topo_gen == o.topo_gen && cls_bound == o.cls_bound; } };
+
+// What one solve leaves the next about the fused solo kernel (fused.cuh).  A solo solve that finds the class set of the
+// previous one keeps its class table, and the next solo solve runs the speculative variant on it.  kept_fp = the
+// class-set fingerprint of the last non-speculative solo solve (0: none -- nothing to compare with, as after a
+// speculative solve missed): speculation resumes only after two such solves in a row agree.
+struct SoloTables {
+  bool hint = true;  // the last batch consisted of data-parallel components only
+  CleanSig clean;
+  bool clean_valid = false;
+  KeptSig kept;
+  bool kept_valid = false;
+  unsigned long long kept_fp = 0;
+
+  // The variant of an attempt; `fused`: the fused kernel may take the batch, `now`: the scratch, topology and class
+  // bound it would run on, `spec_ok`: the batch fits the speculative variant.  Whatever runs dirties the scratch, and
+  // anything but the speculative variant rebuilds or clears the kept table.
+  SolveVariant Choose(bool fused, const KeptSig& now, bool spec_ok) {
+    const SolveVariant v = !fused ? kPipeline : !hint ? kFused
+                         : kept_valid && kept == now && spec_ok ? kSoloSpec
+                         : clean_valid && clean == now.clean ? kSoloClean : kSolo;
+    clean_valid = false;
+    if (v != kSoloSpec) kept_valid = false;
+    return v;
+  }
+  // After an attempt of `v` on `now`: `meta` = the class table's meta words (meta[1]: the flag), `fp` = the solo
+  // kernel's class-set fingerprint.
+  void Take(SolveVariant v, const uint32_t* meta, const KeptSig& now, unsigned long long fp) {
+    if (meta[1] == yd::kFlagSpecMiss) {
+      // the kernel left the scratch clean; the replay builds the table again
+      kept_valid = false;
+      kept_fp = 0;
+      clean = now.clean;
+      clean_valid = true;
+    } else if (meta[1] == 4) {  // a component the solo kernel cannot decide: the general sequence, now and next time
+      hint = false;
+    } else if (meta[1] == 0 && v == kFused) {
+      hint = meta[4] == 0;  // back to one launch when nothing is coupled any more
+    } else if (meta[1] == 0 && (v == kSolo || v == kSoloClean)) {
+      // the kernel's last block has kept the class table (same class set as the previous such solve) or cleared it,
+      // and re-initialised the rest of the scratch.  (A completed speculative solve leaves the kept table valid.)
+      if (fp == kept_fp) {
+        kept = now;
+        kept_valid = true;
+      } else {
+        clean = now.clean;
+        clean_valid = true;
+      }
+      kept_fp = fp;
+    }
+  }
+  // Another sequence (the sharded solve) dirtied the scratch and overwrote the class table.
+  void Drop() { clean_valid = kept_valid = false; }
+};
+
 }  // namespace
 
 struct yd_shard_ctx;  // range-sharded queue over several GPUs (shard_host.inc)
@@ -191,16 +270,16 @@ struct yd_sched {
   // merge solver (solve_merge.cuh): per-slot verdicts and the chunk boundary states
   DevBuf d_slot_pick, d_mst_in, d_mst_out, d_stream_scratch;
   size_t z_merge_off = 0, z_layout_off = 0, z_final_off = 0, z_scan_off = 0;
-  uint32_t merge_chunk = 512, merge_rounds = 16, merge_max_chunks = 0, merge_grid = 0, merge_grid_kcap = 0;
-  bool merge_chunk_auto = true;  // no YDSCHED_MERGE_CHUNK: 256 slots per chunk up to 262 144 requests, 512 above
-  uint32_t stream_debug = 0;   // YDSCHED_STREAM_DEBUG, read once at yd_create
-  uint32_t force_stream = 0;   // yd_config.reserved bit 1 / YDSCHED_FORCE_STREAM: no merge solver for self-requests
-  bool dump_env = false, debug_env = false, tiny_ok = true;
+  uint32_t merge_max_chunks = 0, merge_grid = 0, merge_grid_kcap = 0;
+  // configured at yd_create; a solve starts from these and escalates in its own SolvePlan
+  uint32_t cfg_merge_chunk = 0;    // YDSCHED_MERGE_CHUNK (0: by batch size, MergeChunk)
+  uint32_t cfg_merge_rounds = 16;  // YDSCHED_MERGE_ROUNDS
+  uint32_t cfg_force_stream = 0;   // yd_config.reserved bit 1 / YDSCHED_FORCE_STREAM: no merge solver for self-requests
+  bool debug_env = false, tiny_ok = true;
   bool stream_attr_set = false;
   // fused front kernel (fused.cuh): one persistent launch for the class / rank / list phases and -- `solo` -- the grants
   bool fused_cfg = true;       // yd_config.reserved bit 3 / YDSCHED_NO_FUSED switch it off
-  bool solo_hint = true;       // the last batch consisted of data-parallel components only
-  uint32_t fused_grid = 0;     // blocks of the fused kernel: one per SM
+  uint32_t fused_grid = 0;    // blocks of the fused kernel: one per SM
   uint32_t fused_max_nb = 262144;  // largest batch size class that takes it (YDSCHED_FUSED_MAX_N)
   size_t z_fbar_off = 0;
   DevBuf d_reqs16, d_out8;     // packed upload / download (yd_task_req16, yd_grant8)
@@ -209,24 +288,8 @@ struct yd_sched {
   yd::FusedScalars fsc{};            // the call's scalars: kernel parameters of a solo launch ...
   PinBuf h_fsc;                      // ... or (graphed general sequence) copied into d_fsc by the graph's first node
   DevBuf d_fsc;
-  // The solo kernel re-initialises the scratch it dirtied (class-table keys, zeroed region) before it ends; while this
-  // signature matches the current buffers and layout the next solo solve needs no memset nodes either.
-  struct CleanSig { unsigned long long gen = ~0ull; size_t z_cls_off = 0, z_bytes = 0, res_words = 0; const void* zero = nullptr; const void* res = nullptr;
-    bool operator==(const CleanSig& o) const { return gen == o.gen && z_cls_off == o.z_cls_off && z_bytes == o.z_bytes && res_words == o.res_words && zero == o.zero && res == o.res; } };
-  CleanSig clean_sig;
-  bool clean_valid = false;
-  // A solo solve that finds the class set of the previous one keeps its class table (fused.cuh); the next solo solve
-  // then runs the speculative variant on it, while the buffers, the topology and the class bound are those it was built
-  // with.  kept_fp = the class-set fingerprint of the last non-speculative solo solve (0: none -- nothing to compare
-  // with, as after a speculative solve missed): speculation resumes only after two such solves in a row agree.
-  struct KeptSig { CleanSig clean; unsigned long long topo_gen = 0; uint32_t cls_bound = 0;
-    bool operator==(const KeptSig& o) const { return clean == o.clean && topo_gen == o.topo_gen && cls_bound == o.cls_bound; } };
-  KeptSig kept_sig;
-  bool kept_valid = false;
-  unsigned long long kept_fp = 0;
-  bool fused_lite = true;     // YDSCHED_FUSED_NOLITE: the solo kernel's second barrier keeps its leader scans
-  bool zero_copy = true;       // YDSCHED_NO_ZEROCOPY: page-locked caller arrays are copied like pageable ones
-  bool fused_prof = false;     // YDSCHED_FUSED_PROF: phase stamps of the fused kernel, printed after every solve
+  SoloTables solo;
+  bool fused_prof = false;    // YDSCHED_FUSED_PROF: phase stamps of the fused kernel, printed after every solve
   DevBuf d_fused_prof;
   size_t res_words = 0;  // u32 words of res[] in d_res (the class-table keys follow)
   size_t staged_n = 0;   // requests placed in d_reqs by yd_stage_requests
@@ -252,7 +315,8 @@ struct yd_sched {
   // captured solve graphs, keyed by size class
   struct GraphKey {
     uint32_t Nb = 0, S = 0, n_comps = 0, max_comp = 0, cls_bound = 0, solver = 0, wide = 0, merge_rounds = 0, force_stream = 0,
-             order_static = 0, variant = 0, packed = 0;
+             order_static = 0, packed = 0;
+    SolveVariant variant = kPipeline;
     size_t slot_b = 0;
     unsigned long long gen = 0, topo_gen = 0;  // buffer reallocations; topology rebuilds (n_envs, n_ips, ... are baked in)
     uint64_t ring_cap = 0;
@@ -277,9 +341,7 @@ struct yd_sched {
   yd::FusedArgs last_fused{};  // what LaunchFused passed last (picked up right after a capture)
   uint32_t last_fused_grid = 0;
   size_t last_fused_dyn = 0;
-  bool report_dev = false;     // YDSCHED_REPORT_DEV: the solo kernel's report goes to HBM + a copy node (comparison)
   bool host_prof = false;      // YDSCHED_HOST_PROF: host-side timestamps of a solve, printed
-  DevBuf d_report;
   std::vector<GraphEntry> graphs;
   unsigned long long topo_gen = 0;
   bool use_graphs = true;
@@ -595,21 +657,16 @@ yd_sched* yd_create(const yd_config* cfg) {
   s->id_stride = cfg->id_stride ? cfg->id_stride : 1;
   s->id_offset = cfg->id_stride ? cfg->id_offset : 0;
   s->use_graphs = !(cfg->reserved & 1u) && !getenv("YDSCHED_NO_GRAPH");
-  s->force_stream = ((cfg->reserved & 2u) || getenv("YDSCHED_FORCE_STREAM")) ? 1u : 0u;
-  if (const char* e = getenv("YDSCHED_STREAM_DEBUG")) s->stream_debug = (uint32_t)atoi(e);
-  if (const char* e = getenv("YDSCHED_MERGE_CHUNK")) { s->merge_chunk = std::max(32u, (uint32_t)atoi(e) & ~31u); s->merge_chunk_auto = false; }
-  if (const char* e = getenv("YDSCHED_MERGE_ROUNDS")) s->merge_rounds = std::max(2u, (uint32_t)atoi(e));
+  s->cfg_force_stream = ((cfg->reserved & 2u) || getenv("YDSCHED_FORCE_STREAM")) ? 1u : 0u;
+  if (const char* e = getenv("YDSCHED_MERGE_CHUNK")) s->cfg_merge_chunk = std::max(32u, (uint32_t)atoi(e) & ~31u);
+  if (const char* e = getenv("YDSCHED_MERGE_ROUNDS")) s->cfg_merge_rounds = std::max(2u, (uint32_t)atoi(e));
   s->tiny_ok = !(cfg->reserved & 4u) && !getenv("YDSCHED_NO_TINY");
   s->fused_cfg = !(cfg->reserved & 8u) && !getenv("YDSCHED_NO_FUSED");
   if (const char* e = getenv("YDSCHED_FUSED_MAX_N")) s->fused_max_nb = (uint32_t)std::max(1024, atoi(e));
   YD_CUDA_CHECK(cudaHostAlloc(reinterpret_cast<void**>(&s->h_fio), sizeof(yd::FusedHostIO), cudaHostAllocMapped));
   memset(s->h_fio, 0, sizeof(yd::FusedHostIO));
   YD_CUDA_CHECK(cudaHostGetDevicePointer(reinterpret_cast<void**>(&s->d_fio), s->h_fio, 0));
-  s->zero_copy = getenv("YDSCHED_NO_ZEROCOPY") == nullptr;
-  s->fused_lite = getenv("YDSCHED_FUSED_NOLITE") == nullptr;
-  s->report_dev = getenv("YDSCHED_REPORT_DEV") != nullptr;
   s->host_prof = getenv("YDSCHED_HOST_PROF") != nullptr;
-  s->d_report.ensure(sizeof(yd::FusedHostIO));
   s->fused_prof = getenv("YDSCHED_FUSED_PROF") != nullptr;
   {
     int sms = 0, per_sm = 0;
@@ -623,7 +680,6 @@ yd_sched* yd_create(const yd_config* cfg) {
     s->d_fused_prof.ensure(prof_bytes);
     YD_CUDA_CHECK(cudaMemset(s->d_fused_prof.p, 0, prof_bytes));
   }
-  s->dump_env = getenv("YDSCHED_DUMP") != nullptr;
   s->debug_env = getenv("YDSCHED_DEBUG") != nullptr;
   YD_CUDA_CHECK(cudaStreamCreateWithFlags(&s->st, cudaStreamNonBlocking));
   YD_CUDA_CHECK(cudaStreamCreateWithFlags(&s->st2, cudaStreamNonBlocking));
@@ -665,7 +721,7 @@ void yd_destroy(yd_sched* s) {
                     &s->d_codes, &s->d_ids, &s->d_ok, &s->d_counters, &s->d_sv_env_off, &s->d_sv_envs,
                     &s->d_comp_mode, &s->d_sv_emask, &s->d_slot_rec, &s->d_slot_spos, &s->d_slot_owner, &s->d_sort_k[0], &s->d_sort_k[1], &s->d_sort_v[0],
                     &s->d_sort_v[1], &s->d_zero, &s->d_list, &s->d_list_bal, &s->d_members, &s->d_rcls, &s->d_rrank, &s->d_rank_cnt, &s->d_rq, &s->d_rself,
-                    &s->d_slot_pick, &s->d_mst_in, &s->d_mst_out, &s->d_stream_scratch, &s->d_reqs16, &s->d_out8, &s->d_fused_prof, &s->d_report, &s->d_bloom,
+                    &s->d_slot_pick, &s->d_mst_in, &s->d_mst_out, &s->d_stream_scratch, &s->d_reqs16, &s->d_out8, &s->d_fused_prof, &s->d_bloom,
                     &s->d_bloom_keys, &s->d_bloom_out, &s->d_rt_bytes, &s->d_rt_off, &s->d_rt_len, &s->d_rt_ids,
                     &s->d_rt_slots, &s->d_rt_keys, &s->d_rt_out}) {
     b->release();
@@ -757,7 +813,7 @@ yd::TopoView MakeTopo(yd_sched* s) {
   return t;
 }
 
-yd::ClassTable MakeClassTable(yd_sched* s) {
+yd::ClassTable MakeClassTable(yd_sched* s, const SolvePlan& plan) {
   uint32_t* u = reinterpret_cast<uint32_t*>(static_cast<char*>(s->d_zero.p) + s->z_cls_off);
   yd::ClassTable ct{};
   // the 8-byte keys sit right behind res[] so one 0xFF memset initialises both
@@ -776,7 +832,7 @@ yd::ClassTable MakeClassTable(yd_sched* s) {
   ct.merge_comp = u;                     u += yd::kMaxClasses;
   ct.comp_cls = u;                       // [cls_bound * 32], the tail of the class region
   ct.cls_bound = s->cls_bound;
-  ct.force_stream = s->force_stream;
+  ct.force_stream = plan.force_stream;
   return ct;
 }
 
@@ -898,6 +954,14 @@ uint32_t LaunchSort(yd_sched* s, int first_bit, int last_bit) {
   return launches;
 }
 
+// Merge-solver chunk: more, shorter chunks pay while the request-side passes are short (measured on an H100 SXM, 700 W:
+// cfg2-random 324 vs 374 us, cfg-self 177 vs 187 us at 256 vs 512 slots; cfg3, 1 M requests, 604 vs 573 us).  A sharded
+// solve keeps one length whatever each rank's batch.
+uint32_t MergeChunk(const yd_sched* s, uint32_t Nb) {
+  if (s->cfg_merge_chunk) return s->cfg_merge_chunk;
+  return !s->shard && Nb <= 262144 ? 256u : 512u;
+}
+
 // Allocates everything the slot-stream sequence touches for size class (Nb, slot_b) and
 // lays out the zero-initialised scratch region; called before a graph capture so that no
 // allocation happens inside it.
@@ -942,7 +1006,7 @@ void PrepareStreamBuffers(yd_sched* s, uint32_t Nb, size_t slot_b) {
   s->d_stream_scratch.ensure(std::max<size_t>(s->sv.size(), 1) * 8);
   s->d_slot_pick.ensure(slot_b * 4 * 4);  // one word per list entry
   // every slot is in at most one pseudo-class list: chunks <= slots / chunk + one partial chunk per list
-  s->merge_max_chunks = (uint32_t)(slot_b / s->merge_chunk) + s->cls_bound + 1;
+  s->merge_max_chunks = (uint32_t)(slot_b / MergeChunk(s, Nb)) + s->cls_bound + 1;
   s->d_mst_in.ensure(size_t(s->merge_max_chunks) * yd::kMergeStateWords * 4);
   s->d_mst_out.ensure(size_t(s->merge_max_chunks) * yd::kMergeStateWords * 4);
   s->d_rank_cnt.ensure((size_t(s->cls_bound) * n_rtiles + 1) * 4);
@@ -954,7 +1018,7 @@ void PrepareStreamBuffers(yd_sched* s, uint32_t Nb, size_t slot_b) {
 
 // The merge solver: ONE persistent launch (rounds, scatter and check are phases behind grid barriers), so the
 // grid must be co-resident: occupancy x SMs blocks at most, each looping over its chunks.
-uint32_t LaunchMerge(yd_sched* s, yd::MergeArgs& m, cudaStream_t st) {
+uint32_t LaunchMerge(yd_sched* s, uint32_t Nb, yd::MergeArgs& m, cudaStream_t st) {
   m.kcap = std::min(32u, s->cls_bound);
   const size_t dyn = size_t(1 + m.kcap) * yd::kRingRecs * sizeof(uint2);
   if (s->merge_grid_kcap != m.kcap) {
@@ -964,7 +1028,7 @@ uint32_t LaunchMerge(yd_sched* s, yd::MergeArgs& m, cudaStream_t st) {
     s->merge_grid = (uint32_t)std::max(1, std::min(per_sm, 16) * sms);
     s->merge_grid_kcap = m.kcap;
   }
-  m.chunk = s->merge_chunk;
+  m.chunk = MergeChunk(s, Nb);
   m.max_chunks = s->merge_max_chunks;
   m.diag = &s->d_counters.as<Counters>()->pad[0];
   m.rq_blocks = (uint32_t)(s->d_rq.cap / 256);
@@ -1004,11 +1068,11 @@ uint32_t RebuildSlotOrder(yd_sched* s, size_t slot_b) {
 
 // The solvers for everything the data-parallel path does not decide: the merge solver (all components but those with
 // several servants behind one requestor IP), then the sequential slot-stream walk for the rest.
-uint32_t LaunchCoupledSolvers(yd_sched* s, uint32_t N, size_t slot_b, const yd::RqLayout& L) {
+uint32_t LaunchCoupledSolvers(yd_sched* s, uint32_t N, size_t slot_b, const SolvePlan& plan, const yd::RqLayout& L) {
   cudaStream_t st = s->st;
   uint32_t launches = 0;
   yd::TopoView t = MakeTopo(s);
-  yd::ClassTable ct = MakeClassTable(s);
+  yd::ClassTable ct = MakeClassTable(s, plan);
   yd::ServantArrays arr = s->arrays();
   const yd::DynParams* dp = s->d_dyn.as<yd::DynParams>();
   uint32_t* list_cnt = reinterpret_cast<uint32_t*>(static_cast<char*>(s->d_zero.p) + s->z_listcnt_off);
@@ -1027,7 +1091,7 @@ uint32_t LaunchCoupledSolvers(yd_sched* s, uint32_t N, size_t slot_b, const yd::
     m.st_in = s->d_mst_in.as<uint32_t>(); m.st_out = s->d_mst_out.as<uint32_t>();
     m.res = s->d_res.as<uint32_t>();
     m.L = L;
-    launches += LaunchMerge(s, m, st);
+    launches += LaunchMerge(s, N, m, st);
   }
 
   // ---- sequential decisions for everything else ---------------------------------------------
@@ -1049,7 +1113,6 @@ uint32_t LaunchCoupledSolvers(yd_sched* s, uint32_t N, size_t slot_b, const yd::
   a.comp_mode = s->d_comp_mode.as<uint32_t>();
   a.viol = mp.viol;
   a.counters = s->d_counters.as<Counters>();
-  a.debug = s->stream_debug;
   const size_t dyn = size_t(a.max_comp_servants) * 8;
   yd::k_solve_stream<<<s->n_comps, (yd::kStreamProducers + 1) * 32, dyn, st>>>(a);
   launches += 1;
@@ -1061,11 +1124,11 @@ uint32_t LaunchCoupledSolvers(yd_sched* s, uint32_t N, size_t slot_b, const yd::
 //   st2 : [wait for the request upload] class table -> finalize -> FIFO ranks -> scan
 // joined before the per-class lists.  `capturing` selects the external-event flavour of
 // the wait on the upload (the upload itself is never part of the graph).
-uint32_t LaunchStream(yd_sched* s, uint32_t N, size_t slot_b, bool capturing) {
+uint32_t LaunchStream(yd_sched* s, uint32_t N, size_t slot_b, const SolvePlan& plan, bool capturing) {
   cudaStream_t st = s->st, st2 = s->st2;
   uint32_t launches = 0;
   yd::TopoView t = MakeTopo(s);
-  yd::ClassTable ct = MakeClassTable(s);
+  yd::ClassTable ct = MakeClassTable(s, plan);
   yd::ServantArrays arr = s->arrays();
   const yd::DynParams* dp = s->d_dyn.as<yd::DynParams>();
   uint32_t* list_cnt = reinterpret_cast<uint32_t*>(static_cast<char*>(s->d_zero.p) + s->z_listcnt_off);
@@ -1120,16 +1183,23 @@ uint32_t LaunchStream(yd_sched* s, uint32_t N, size_t slot_b, bool capturing) {
                                                      s->d_rq.as<uint2>(), s->d_res.as<uint32_t>(), L);
   launches += 1;
 
-  launches += LaunchCoupledSolvers(s, N, slot_b, L);
+  launches += LaunchCoupledSolvers(s, N, slot_b, plan, L);
   return launches;
 }
 
-constexpr size_t kFusedLoffCacheWords = 16384;  // 64 KB of dynamic shared memory at most
+// The solo kernel searches the scanned list offsets, cls_bound x (slot tiles + 1) + 1 words, once per request.  When they
+// fit in dynamic shared memory (64 KB at most) every block derives the offsets it needs from the raw counts, without
+// the leader scans of E2 (fused.cuh); the speculative variant needs that.  Returns the words, 0 when they do not fit.
+uint32_t FusedLoffWords(const yd_sched* s, size_t slot_b) {
+  const size_t cells = size_t(s->cls_bound) * ((slot_b + yd::kListTile - 1) / yd::kListTile + 1) + 1;
+  return cells <= 16384 ? (uint32_t)cells : 0u;
+}
 
 // The fused front (fused.cuh): classes, ranks, lists and the data-parallel verdicts in ONE persistent launch on `st`;
-// `solo`: grants, task ids and leases too (batches made of data-parallel components only), else the coupled solvers
-// follow.  Needs the kept slot order.
-uint32_t LaunchFused(yd_sched* s, uint32_t N, size_t slot_b, bool capturing, bool solo, bool spec, bool packed_in, bool packed_out) {
+// solo variants: grants, task ids and leases too (batches made of data-parallel components only), else the coupled
+// solvers follow.  Needs the kept slot order.
+uint32_t LaunchFused(yd_sched* s, uint32_t N, size_t slot_b, const SolvePlan& plan, bool capturing, bool packed_in, bool packed_out) {
+  const bool solo = IsSolo(plan.variant);
   cudaStream_t st = s->st;
   uint32_t launches = 0;
   const uint32_t n_tiles = (uint32_t)((slot_b + yd::kListTile - 1) / yd::kListTile);
@@ -1139,7 +1209,7 @@ uint32_t LaunchFused(yd_sched* s, uint32_t N, size_t slot_b, bool capturing, boo
   // graphed general sequence: the scalars come through a copy node; a solo graph gets them as (patched) kernel parameters
   a.sc_dev = (capturing && !solo) ? s->d_fsc.as<yd::FusedScalars>() : nullptr;
   if (a.sc_dev) YD_CUDA_CHECK(cudaMemcpyAsync(s->d_fsc.p, s->h_fsc.p, sizeof(yd::FusedScalars), cudaMemcpyHostToDevice, st));
-  a.hio = s->report_dev ? s->d_report.as<yd::FusedHostIO>() : s->d_fio;
+  a.hio = s->d_fio;
   a.dyn_out = solo ? nullptr : s->d_dyn.as<yd::DynParams>();
   a.clean_keys = reinterpret_cast<unsigned long long*>(s->d_res.as<uint32_t>() + s->res_words);
   a.clean_zero = reinterpret_cast<uint4*>(static_cast<char*>(s->d_zero.p) + s->z_cls_off);
@@ -1149,7 +1219,7 @@ uint32_t LaunchFused(yd_sched* s, uint32_t N, size_t slot_b, bool capturing, boo
   a.reqs16_w = packed_in ? s->d_reqs16.as<uint4>() : nullptr;
   a.reqs_w = (packed_in && !solo) ? s->d_reqs.as<yd_task_req>() : nullptr;
   a.t = MakeTopo(s);
-  a.ct = MakeClassTable(s);
+  a.ct = MakeClassTable(s, plan);
   a.sv = s->arrays();
   a.dec = yd::SlotDecode{s->d_sort_v[0].as<uint32_t>(), s->d_slot_owner.as<uint32_t>(), s->d_row_off.as<uint32_t>(),
                          s->d_row_len.as<uint32_t>(), s->d_run.as<uint32_t>(), 1u, s->d_slot_rec.as<uint2>()};
@@ -1181,12 +1251,9 @@ uint32_t LaunchFused(yd_sched* s, uint32_t N, size_t slot_b, bool capturing, boo
   a.prof = s->fused_prof ? s->d_fused_prof.as<unsigned long long>() : nullptr;
   YD_CUDA_CHECK(cudaStreamWaitEvent(st, s->ev_h2d, capturing ? cudaEventWaitExternal : 0));
   const uint32_t grid = s->fused_grid;  // one block per SM, whatever the batch: the phases hand out tiles of two kinds
-  // solo: the scanned list offsets are searched once per request -- from shared memory when they fit
-  const size_t cells = size_t(s->cls_bound) * (n_tiles + 1) + 1;
-  const size_t dyn = solo && cells <= kFusedLoffCacheWords ? cells * 4 : 0;
-  a.loff_cache_words = (uint32_t)(dyn / 4);
-  a.lite = s->fused_lite ? 1u : 0u;
-  a.spec = spec ? 1u : 0u;
+  a.loff_cache_words = solo ? FusedLoffWords(s, slot_b) : 0u;
+  const size_t dyn = size_t(a.loff_cache_words) * 4;
+  a.spec = plan.variant == kSoloSpec ? 1u : 0u;
   a.kept_env = s->d_kept_env.as<uint4>();
   a.kept_sv = s->d_kept_sv.as<uint32_t>();
   a.slot_spos = s->d_slot_spos.as<uint32_t>();
@@ -1194,11 +1261,8 @@ uint32_t LaunchFused(yd_sched* s, uint32_t N, size_t slot_b, bool capturing, boo
   s->last_fused = a;
   s->last_fused_grid = grid;
   s->last_fused_dyn = dyn;
-  if (solo && s->report_dev) {
-    YD_CUDA_CHECK(cudaMemcpyAsync(s->h_fio, s->d_report.p, sizeof(yd::FusedHostIO), cudaMemcpyDeviceToHost, st));
-  }
   launches += 1;
-  if (!solo) launches += LaunchCoupledSolvers(s, N, slot_b, a.L);
+  if (!solo) launches += LaunchCoupledSolvers(s, N, slot_b, plan, a.L);
   return launches;
 }
 
@@ -1216,26 +1280,25 @@ uint64_t NextPow2(uint64_t v, uint64_t lo) {
 
 // Everything between the request upload and the grant download, for size class
 // (Nb, slot_b): the sequence that is captured into a CUDA graph.
-// variant: 0 = the kernel-by-kernel pipeline, 1 = fused front + coupled solvers + final, 2 = fused front alone (solo),
-// 3 = the same on a clean scratch (no memset nodes), 4 = solo and speculative on the kept class table (no memsets).
 // packed bit 0: the upload is 16-byte records in d_reqs16; bit 1: the download is 8-byte grants from d_out8.
-uint32_t EnqueueSolve(yd_sched* s, uint32_t Nb, size_t slot_b, uint32_t solver, bool record_events, bool capturing,
-                      uint32_t variant = 0, uint32_t packed = 0) {
+uint32_t EnqueueSolve(yd_sched* s, uint32_t Nb, size_t slot_b, const SolvePlan& plan, bool record_events, bool capturing,
+                      uint32_t packed) {
   cudaStream_t st = s->st;
   const uint32_t S = (uint32_t)s->sv.size();
+  const uint32_t solver = plan.solver;
   const bool have_work = S && s->n_comps;
   const uint32_t nb = (Nb + 1023) / 1024;
   const bool packed_in = packed & 1u, packed_out = packed & 2u;
   uint32_t launches = 0;
   const yd::DynParams* dp = s->d_dyn.as<yd::DynParams>();
-  const bool fused = variant && have_work && solver == 2;
-  const bool solo = fused && variant >= 2;
+  const bool fused = plan.variant != kPipeline && have_work && solver == 2;
+  const bool solo = fused && IsSolo(plan.variant);
   // (the fused kernel reads the call's scalars from the mapped host record and -- not solo -- stores them in d_dyn itself)
   if (!fused) YD_CUDA_CHECK(cudaMemcpyAsync(s->d_dyn.p, s->h_dyn.p, sizeof(yd::DynParams), cudaMemcpyHostToDevice, st));
   if (solo) {
     // the solo kernel keeps the verdicts in registers: only the class-table keys behind res[] are initialised -- and
-    // not even those (variant 3) when the previous solo solve left the scratch clean
-    if (variant == 2) {
+    // not even those when the previous solo solve left the scratch clean
+    if (plan.variant == kSolo) {
       YD_CUDA_CHECK(cudaMemsetAsync(s->d_res.as<uint32_t>() + s->res_words, 0xFF, yd::kClsTableSize * 8, st));
       YD_CUDA_CHECK(cudaMemsetAsync(static_cast<char*>(s->d_zero.p) + s->z_cls_off, 0, s->z_bytes - s->z_cls_off, st));
     }
@@ -1246,7 +1309,7 @@ uint32_t EnqueueSolve(yd_sched* s, uint32_t Nb, size_t slot_b, uint32_t solver, 
   }
   if (record_events) YD_CUDA_CHECK(cudaEventRecord(s->ev[1], st));
   const uint32_t* abort_flag = nullptr;
-  if (packed_in && !(variant && have_work && solver == 2)) {
+  if (packed_in && !fused) {
     // 16-byte upload -> the 24-byte queue the pipeline kernels read
     YD_CUDA_CHECK(cudaStreamWaitEvent(st, s->ev_h2d, capturing ? cudaEventWaitExternal : 0));
     yd::k_unpack_reqs<<<(Nb + 255) / 256, 256, 0, st>>>(s->d_reqs16.as<uint4>(), dp, s->d_reqs.as<yd_task_req>());
@@ -1254,9 +1317,9 @@ uint32_t EnqueueSolve(yd_sched* s, uint32_t Nb, size_t slot_b, uint32_t solver, 
   }
   if (have_work && solver == 2) {
     if (record_events) YD_CUDA_CHECK(cudaEventRecord(s->ev[2], st));
-    if (variant) launches += LaunchFused(s, Nb, slot_b, capturing, variant >= 2, variant == 4, packed_in, packed_out);
-    else launches += LaunchStream(s, Nb, slot_b, capturing);
-    abort_flag = MakeClassTable(s).meta + 1;
+    if (fused) launches += LaunchFused(s, Nb, slot_b, plan, capturing, packed_in, packed_out);
+    else launches += LaunchStream(s, Nb, slot_b, plan, capturing);
+    abort_flag = MakeClassTable(s, plan).meta + 1;
   } else {
     if (have_work) launches += LaunchSlotTable(s, false);
     if (record_events) YD_CUDA_CHECK(cudaEventRecord(s->ev[2], st));
@@ -1301,70 +1364,6 @@ uint32_t EnqueueSolve(yd_sched* s, uint32_t Nb, size_t slot_b, uint32_t solver, 
   return launches;
 }
 
-
-// Debug aid (YDSCHED_DUMP=1): hashes of every intermediate of the slot-stream pipeline after a
-// solve, to compare two runs stage by stage.
-void DumpStreamState(yd_sched* s, uint32_t Nb, size_t slot_b) {
-  static int solve_no = 0;
-  ++solve_no;
-  auto fetch = [&](const void* p, size_t bytes) {
-    std::vector<unsigned char> h(bytes);
-    if (bytes) YD_CUDA_CHECK(cudaMemcpy(h.data(), p, bytes, cudaMemcpyDeviceToHost));
-    return h;
-  };
-  auto hash = [&](const char* name, const std::vector<unsigned char>& h) {
-    unsigned long long x = 1469598103934665603ull;
-    for (unsigned char c : h) { x ^= c; x *= 1099511628211ull; }
-    fprintf(stderr, "YDDUMP %d %-12s %8zu %016llx\n", solve_no, name, h.size(), x);
-  };
-  Counters c;
-  YD_CUDA_CHECK(cudaMemcpy(&c, s->d_counters.p, sizeof c, cudaMemcpyDeviceToHost));
-  const size_t m = (size_t)c.slots, ksz = s->wide ? 8 : 4;
-  const uint32_t S = (uint32_t)s->sv.size();
-  fprintf(stderr, "YDDUMP %d slots %zu Nb %u slot_b %zu cls_bound %u\n", solve_no, m, Nb, slot_b, s->cls_bound);
-  hash("row_off", fetch(s->d_row_off.p, size_t(S + 1) * 4));
-  hash("row_len", fetch(s->d_row_len.p, size_t(S) * 4));
-  hash("codes", fetch(s->d_codes.p, m * ksz));
-  hash("owner", fetch(s->d_slot_owner.p, m * 4));
-  hash("sorted_k", fetch(s->d_sort_k[0].p, m * ksz));
-  hash("sorted_v", fetch(s->d_sort_v[0].p, m * 4));
-  yd::ClassTable ct = MakeClassTable(s);
-  auto meta = fetch(ct.meta, 32);
-  const uint32_t* mt = reinterpret_cast<const uint32_t*>(meta.data());
-  fprintf(stderr, "YDDUMP %d meta %u %u %u %u\n", solve_no, mt[0], mt[1], mt[2], mt[3]);
-  const uint32_t ncls = std::min(mt[0], yd::kMaxClasses);
-  hash("cls_env", fetch(ct.cls_env, ncls * 4));
-  hash("cls_mv", fetch(ct.cls_mv, ncls * 4));
-  hash("cls_nelig", fetch(ct.cls_nelig, ncls * 4));
-  hash("comp_mode", fetch(s->d_comp_mode.p, size_t(s->n_comps) * 4));
-  const uint32_t n_tiles = (uint32_t)((slot_b + yd::kListTile - 1) / yd::kListTile);
-  auto lo = fetch(static_cast<char*>(s->d_zero.p) + s->z_listcnt_off, (size_t(mt[3]) * n_tiles + 1) * 4);
-  hash("list_off", lo);
-  const uint32_t total = reinterpret_cast<const uint32_t*>(lo.data())[size_t(mt[3]) * n_tiles];
-  fprintf(stderr, "YDDUMP %d list_total %u\n", solve_no, total);
-  hash("list", fetch(s->d_list.p, size_t(total) * 8));
-  hash("res", fetch(s->d_res.p, size_t(s->h_dyn.as<yd::DynParams>()->n) * 4));
-  hash("run_after", fetch(s->d_run.p, size_t(S) * 4));
-  if (const char* dir = getenv("YDSCHED_DUMP_DIR")) {
-    auto save = [&](const char* name, const std::vector<unsigned char>& h) {
-      char path[512];
-      snprintf(path, sizeof path, "%s/s%d_%s.bin", dir, solve_no, name);
-      if (FILE* f = fopen(path, "wb")) { fwrite(h.data(), 1, h.size(), f); fclose(f); }
-    };
-    save("sorted_k", fetch(s->d_sort_k[0].p, m * ksz));
-    save("sorted_v", fetch(s->d_sort_v[0].p, m * 4));
-    save("owner", fetch(s->d_slot_owner.p, m * 4));
-    save("row_off", fetch(s->d_row_off.p, size_t(S + 1) * 4));
-    save("row_len", fetch(s->d_row_len.p, size_t(S) * 4));
-    save("list_off", lo);
-    save("list", fetch(s->d_list.p, size_t(total) * 8));
-    save("cls_env", fetch(ct.cls_env, ncls * 4));
-    save("cls_mv", fetch(ct.cls_mv, ncls * 4));
-    save("res", fetch(s->d_res.p, size_t(s->h_dyn.as<yd::DynParams>()->n) * 4));
-    save("run_after", fetch(s->d_run.p, size_t(S) * 4));
-    save("reqs", fetch(s->d_reqs.p, size_t(s->h_dyn.as<yd::DynParams>()->n) * sizeof(yd_task_req)));
-  }
-}
 }  // namespace
 }  // extern "C++"
 
@@ -1460,9 +1459,6 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
   const uint32_t Nb = (uint32_t)NextPow2(N, 1024);
   // The slot table: kept across solves (all running_tasks values of every servant) while it is small enough,
   // else rebuilt per solve and clamped to the batch size.
-  // Merge-solver chunk: more, shorter chunks pay while the request-side passes are short (measured on an H100 SXM, 700 W:
-  // cfg2-random 324 vs 374 us, cfg-self 177 vs 187 us at 256 vs 512 slots; cfg3, 1 M requests, 604 vs 573 us)
-  if (s->merge_chunk_auto && !s->shard) s->merge_chunk = Nb <= 262144 ? 256u : 512u;
   const size_t static_bound = S ? s->static_bound_cache : 0;  // (= StaticSlotBound(s), kept by SyncFacts)
   const bool want_static = s->solver_pref != 1 && static_bound <= kStaticSlotLimit;
   size_t slot_bound = static_bound;
@@ -1489,8 +1485,9 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
   // solver choice: 2 (slot streams) unless asked otherwise or a component is too big for it
   // (the slot-stream solver takes components of any size: its sequential fallback keeps running_tasks of a
   // component beyond kStreamMaxComponent servants in HBM instead of shared memory)
-  uint32_t solver = s->solver_pref == 1 ? 1 : 2;
-  if (solver == 1 && s->max_comp_servants > kRowscanMaxComponent) solver = 2;  // the row-scan solver holds 8192 servants per component
+  // (the row-scan solver holds 8192 servants per component)
+  SolvePlan plan{kPipeline, s->solver_pref == 1 && s->max_comp_servants <= kRowscanMaxComponent ? 1u : 2u,
+                 s->cfg_merge_rounds, s->cfg_force_stream};
 
   yd::DynParams* hd = s->h_dyn.as<yd::DynParams>();
   hd->n = N;
@@ -1518,7 +1515,7 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
     uploaded = true;
   };
   auto mapped_address = [&](const void* p) -> void* {
-    if (!p || !s->zero_copy || (reinterpret_cast<uintptr_t>(p) & 15u)) return nullptr;  // (16-byte vector accesses)
+    if (!p || (reinterpret_cast<uintptr_t>(p) & 15u)) return nullptr;  // (16-byte vector accesses)
     cudaPointerAttributes at{};
     if (cudaPointerGetAttributes(&at, p) != cudaSuccess) { cudaGetLastError(); return nullptr; }
     return at.type == cudaMemoryTypeHost ? at.devicePointer : nullptr;
@@ -1528,79 +1525,68 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
   void* const out_dev = mapped_address(out ? static_cast<void*>(out) : static_cast<void*>(out8));
   if (in_host) s->staged_n = 0;  // the staging area now holds this batch
   bool graphed = false;
-  const uint32_t merge_rounds_cfg = s->merge_rounds, force_stream_cfg = s->force_stream;
   int merge_retry = 0, grow_attempts = 0;
-  uint32_t variant = 0;
   uint32_t spec = 0;  // the speculative variant: 0 not tried, 1 decided the batch, 2 missed (the batch was replayed)
   for (;;) {
     memset(s->h_meta.p, 0, 32);
     graphed = false;
     // The fused front kernel takes batches in the latency-bound regime whose (class, tile) count matrices one block
-    // scans in a few rounds; it needs the kept slot order.  solo = it also writes the grants (no coupled component
-    // had requests last time; if one has now, the kernel raises flag 4 and the batch is replayed with variant 1).
-    variant = 0;
-    if (s->fused_cfg && s->fused_grid && s->solver_pref == 0 && solver == 2 && want_static && S && s->n_comps && Nb <= s->fused_max_nb &&
-        size_t(s->cls_bound) * ((Nb + yd::kRankTile - 1) / yd::kRankTile) <= 32768 &&
-        size_t(s->cls_bound) * ((slot_b + yd::kListTile - 1) / yd::kListTile) <= 32768) {
-      variant = s->solo_hint ? 2u : 1u;
+    // scans in a few rounds; it needs the kept slot order.  Solo = it also writes the grants (no coupled component
+    // had requests last time; if one has now, the kernel raises flag 4 and the batch is replayed with kFused).
+    const bool fused = s->fused_cfg && s->fused_grid && s->solver_pref == 0 && plan.solver == 2 && want_static && S &&
+                       s->n_comps && Nb <= s->fused_max_nb &&
+                       size_t(s->cls_bound) * ((Nb + yd::kRankTile - 1) / yd::kRankTile) <= 32768 &&
+                       size_t(s->cls_bound) * ((slot_b + yd::kListTile - 1) / yd::kListTile) <= 32768;
+    KeptSig now;
+    if (fused && s->solo.hint) {
+      PrepareStreamBuffers(s, Nb, slot_b);  // (fixes the scratch layout the signature describes)
+      now = KeptSig{CleanSig{g_buf_generation, s->z_cls_off, s->z_bytes, s->res_words, s->d_zero.p, s->d_res.p},
+                    s->topo_gen, s->cls_bound};
     }
-    yd_sched::CleanSig sig_now;
-    if (variant == 2) {
-      if (solver == 2) PrepareStreamBuffers(s, Nb, slot_b);  // (fixes the scratch layout the signature describes)
-      sig_now = yd_sched::CleanSig{g_buf_generation, s->z_cls_off, s->z_bytes, s->res_words, s->d_zero.p, s->d_res.p};
-      // speculative (fused.cuh): the kept class table is the one these buffers, this topology and this class bound
-      // had; every block holds at most two request tiles (their classes and ranks stay in registers), the lists'
-      // offsets fit in shared memory (the selection without leader scans), and registry positions fit the member words
-      // below the slot's index in its tile (classes.cuh: kMemberSlotShift)
-      const size_t lcells = size_t(s->cls_bound) * ((slot_b + yd::kListTile - 1) / yd::kListTile + 1) + 1;
-      if (s->kept_valid && s->kept_sig == yd_sched::KeptSig{sig_now, s->topo_gen, s->cls_bound} && s->fused_lite &&
-          lcells <= kFusedLoffCacheWords && (Nb + yd::kRankTile - 1) / yd::kRankTile <= 2 * s->fused_grid &&
-          S <= yd::kMemberPosMask) {
-        variant = 4;  // the graph is the kernel alone
-      } else if (s->clean_valid && s->clean_sig == sig_now) {
-        variant = 3;  // no memset nodes: the graph is the kernel alone
-      }
-    }
-    s->clean_valid = false;  // (whatever runs now dirties the scratch; a completed solo solve says otherwise below)
-    if (variant != 4) s->kept_valid = false;  // (any other solve rebuilds or clears the class table)
+    // speculative (fused.cuh): every block holds at most two request tiles (their classes and ranks stay in
+    // registers), the lists' offsets fit in shared memory, and registry positions fit the member words below the slot's
+    // index in its tile (classes.cuh: kMemberSlotShift)
+    const bool spec_ok = FusedLoffWords(s, slot_b) != 0 && (Nb + yd::kRankTile - 1) / yd::kRankTile <= 2 * s->fused_grid &&
+                         S <= yd::kMemberPosMask;
+    plan.variant = s->solo.Choose(fused, now, spec_ok);
     // (a staged solve -- no request array in this call -- leaves its grants in HBM and copies them afterwards, so that
     // the device-side events around it time the solve alone)
-    const bool zc_in = variant >= 1 && in_dev, zc_out = variant >= 2 && out_dev && in_host;
+    const bool solo = IsSolo(plan.variant);
+    const bool zc_in = plan.variant != kPipeline && in_dev, zc_out = solo && out_dev && in_host;
     hp[2] = hp_now();
     if (!zc_in) upload();
     YD_CUDA_CHECK(cudaEventRecord(s->ev_h2d, s->st_copy));
     s->fsc.zc_in = zc_in ? in_dev : nullptr;
     s->fsc.zc_out = zc_out ? out_dev : nullptr;
     s->fsc.seq += 1;
-    s->fsc.kept_fp = s->kept_fp;
+    s->fsc.kept_fp = s->solo.kept_fp;
     *s->h_fsc.as<yd::FusedScalars>() = s->fsc;
     s->h_fio->done_seq = 0;
+    // every buffer the sequence touches exists BEFORE a capture (no allocation inside one)
+    if (plan.solver == 2) PrepareStreamBuffers(s, Nb, slot_b);
+    if (plan.solver == 2 && want_static && S && s->n_comps && (s->order_dirty || !s->order_static || s->order_slot_b != slot_b)) {
+      launches += RebuildSlotOrder(s, slot_b);
+    }
     if (s->use_graphs) {
-      // make sure every buffer the sequence touches exists BEFORE capturing (no allocation
-      // inside a capture), then look the size class up
-      if (solver == 2) PrepareStreamBuffers(s, Nb, slot_b);
-      if (solver == 2 && want_static && S && s->n_comps && (s->order_dirty || !s->order_static || s->order_slot_b != slot_b)) {
-        launches += RebuildSlotOrder(s, slot_b);
-      }
       yd_sched::GraphKey key;
       key.Nb = Nb; key.S = S; key.n_comps = s->n_comps; key.max_comp = s->max_comp_servants;
-      key.cls_bound = s->cls_bound; key.solver = solver; key.wide = s->wide; key.slot_b = slot_b;
+      key.cls_bound = s->cls_bound; key.solver = plan.solver; key.wide = s->wide; key.slot_b = slot_b;
       key.gen = g_buf_generation; key.topo_gen = s->topo_gen; key.ring_cap = s->ring_cap;
-      key.merge_rounds = s->merge_rounds; key.force_stream = s->force_stream;
-      key.order_static = (solver == 2 && s->order_static) ? 1u : 0u;
-      key.variant = variant; key.packed = packed;
+      key.merge_rounds = plan.merge_rounds; key.force_stream = plan.force_stream;
+      key.order_static = (plan.solver == 2 && s->order_static) ? 1u : 0u;
+      key.variant = plan.variant; key.packed = packed;
       yd_sched::GraphEntry* hit = nullptr;
       for (auto& g : s->graphs) if (g.key == key) { hit = &g; break; }
       if (!hit) {
         cudaGraph_t graph = nullptr;
         YD_CUDA_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-        uint32_t l = EnqueueSolve(s, Nb, slot_b, solver, false, true, variant, packed);
+        uint32_t l = EnqueueSolve(s, Nb, slot_b, plan, false, true, packed);
         YD_CUDA_CHECK(cudaStreamEndCapture(st, &graph));
         cudaGraphExec_t exec = nullptr;
         YD_CUDA_CHECK(cudaGraphInstantiate(&exec, graph, 0));
         yd_sched::GraphEntry ge;
         ge.key = key; ge.exec = exec; ge.launches = l;
-        if (variant >= 2) {
+        if (solo) {
           // keep the graph: its kernel node is the handle through which the scalars are patched
           size_t nn = 0;
           YD_CUDA_CHECK(cudaGraphGetNodes(graph, nullptr, &nn));
@@ -1627,7 +1613,7 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
         s->graphs.push_back(ge);
         hit = &s->graphs.back();
       }
-      if (variant >= 2) {  // this call's scalars -> the kernel node's parameters
+      if (solo) {  // this call's scalars -> the kernel node's parameters
         hit->fargs.sc = s->fsc;
         void* kp[1] = {&hit->fargs};
         cudaKernelNodeParams np{};
@@ -1647,13 +1633,9 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
       launches += hit->launches;
       graphed = true;
     } else {
-      if (solver == 2) PrepareStreamBuffers(s, Nb, slot_b);
-      if (solver == 2 && want_static && S && s->n_comps && (s->order_dirty || !s->order_static || s->order_slot_b != slot_b)) {
-        launches += RebuildSlotOrder(s, slot_b);
-      }
-      launches += EnqueueSolve(s, Nb, slot_b, solver, true, false, variant, packed);
+      launches += EnqueueSolve(s, Nb, slot_b, plan, true, false, packed);
     }
-    if (solver == 1) { s->order_dirty = true; s->order_static = false; }  // the row-scan solver's table overwrote the kept one
+    if (plan.solver == 1) { s->order_dirty = true; s->order_static = false; }  // the row-scan solver's table overwrote the kept one
     if (zc_out) {}  // the kernel wrote the grants into the caller's page-locked array
     else if (out8) YD_CUDA_CHECK(cudaMemcpyAsync(out8, s->d_out8.p, size_t(N) * sizeof(yd_grant8), cudaMemcpyDeviceToHost, st));
     else YD_CUDA_CHECK(cudaMemcpyAsync(out, s->d_out.p, size_t(N) * sizeof(yd_grant), cudaMemcpyDeviceToHost, st));
@@ -1661,13 +1643,12 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
     hp[5] = hp_now();
     YD_CUDA_CHECK(cudaStreamSynchronize(st));
     hp[6] = hp_now();
-    if (variant >= 2) {  // the solo kernel's report: flags and grant count (there are no copy nodes in its graph)
+    if (solo) {  // the solo kernel's report: flags and grant count (there are no copy nodes in its graph)
       if (s->h_fio->done_seq != s->fsc.seq) { fprintf(stderr, "ydsched: the fused kernel left no report\n"); abort(); }
       memcpy(s->h_meta.p, const_cast<const uint32_t*>(s->h_fio->meta), 32);
       s->h_counters.as<Counters>()->granted = s->h_fio->granted;
     }
-    if (s->dump_env && solver == 2 && S && s->n_comps) DumpStreamState(s, Nb, slot_b);
-    if (s->fused_prof && variant == 4) {
+    if (s->fused_prof && plan.variant == kSoloSpec) {
       unsigned long long t[9];
       YD_CUDA_CHECK(cudaMemcpy(t, s->d_fused_prof.p, sizeof t, cudaMemcpyDeviceToHost));
       if (s->h_meta.as<uint32_t>()[1] == yd::kFlagSpecMiss) {  // (no phase B)
@@ -1684,35 +1665,33 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
       std::string line = "ydsched: fused blocks " + std::to_string(G) + " last_end " + std::to_string(t[8]) + " stamps";
       for (unsigned long long v : b) line += " " + std::to_string(v);
       fprintf(stderr, "%s\n", line.c_str());
-    } else if (s->fused_prof && variant) {
+    } else if (s->fused_prof && plan.variant != kPipeline) {
       unsigned long long t[9];
       YD_CUDA_CHECK(cudaMemcpy(t, s->d_fused_prof.p, sizeof t, cudaMemcpyDeviceToHost));
-      fprintf(stderr, "ydsched: fused variant %u n %u ns: P1 %llu E1 %llu P3 %llu E2 %llu P5 %llu B3 %llu P6 %llu total %llu (+report/clean %lld)\n", variant, N,
-              t[1] - t[0], t[2] - t[1], t[3] - t[2], t[4] - t[3], t[5] - t[4], t[6] - t[5], t[7] - t[6], t[7] - t[0], (long long)(t[8] - t[7]));
+      fprintf(stderr, "ydsched: fused variant %u n %u ns: P1 %llu E1 %llu P3 %llu E2 %llu P5 %llu B3 %llu P6 %llu total %llu (+report/clean %lld)\n",
+              (unsigned)plan.variant, N, t[1] - t[0], t[2] - t[1], t[3] - t[2], t[4] - t[3], t[5] - t[4], t[6] - t[5], t[7] - t[6],
+              t[7] - t[0], (long long)(t[8] - t[7]));
     }
-    if (solver == 2 && S && s->n_comps && s->h_meta.as<uint32_t>()[1] != 0) {
+    const uint32_t* meta = s->h_meta.as<uint32_t>();
+    s->solo.Take(plan.variant, meta, now, s->h_fio->classes_fp);
+    if (plan.solver == 2 && S && s->n_comps && meta[1] != 0) {
       // Nothing was decided (the stream solver and the final kernels all stood down).
-      const uint32_t flag = s->h_meta.as<uint32_t>()[1], ncls = s->h_meta.as<uint32_t>()[0];
+      const uint32_t flag = meta[1], ncls = meta[0];
       if (flag == yd::kFlagSpecMiss) {
-        // the kept class table could not decide the batch and the kernel left the scratch clean: replay without
-        // speculation (which builds the table again), and speculate again only once two solves agree on the class set
+        // the kept class table could not decide the batch: replay without speculation (which builds the table again)
         spec = 2;
-        s->kept_valid = false;
-        s->kept_fp = 0;
-        s->clean_sig = sig_now;
-        s->clean_valid = true;
-      } else if (flag == 4) {  // the solo kernel met a component it cannot decide: the general sequence, now and next time
-        s->solo_hint = false;
+      } else if (flag == 4) {
+        // the solo kernel met a component it cannot decide: the general sequence, now and next time (SoloTables::Take)
       } else if (flag == 2 && grow_attempts++ < 3 && s->cls_bound < yd::kMaxClasses) {  // more lists than provisioned: grow and go again
         // one list per class plus one pseudo-class list per merge-mode component
-        const uint32_t want = ncls + s->h_meta.as<uint32_t>()[2] + 1;
+        const uint32_t want = ncls + meta[2] + 1;
         s->cls_bound *= 2;
         while (s->cls_bound < want && s->cls_bound < yd::kMaxClasses) s->cls_bound *= 2;
       } else if (flag == 3 && merge_retry < 2) {
         // the merge solver's boundary states had not settled after the rounds in the graph: more
         // rounds first, then the sequential solver for everything it would have decided
-        if (merge_retry == 0) s->merge_rounds = std::min(s->merge_rounds * 8, s->merge_max_chunks + 2);
-        else s->force_stream = 2;
+        if (merge_retry == 0) plan.merge_rounds = std::min(plan.merge_rounds * 8, s->merge_max_chunks + 2);
+        else plan.force_stream = 2;
         ++merge_retry;
       } else {
         if (s->max_comp_servants > kRowscanMaxComponent) {
@@ -1720,8 +1699,6 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
           // decisions are the first half's followed by the second half's: decide the batch as two consecutive halves
           // (each with half the requests, hence -- eventually -- few enough classes).
           if (N < 2) { fprintf(stderr, "ydsched: class table overflow on a single request\n"); abort(); }
-          s->merge_rounds = merge_rounds_cfg;
-          s->force_stream = force_stream_cfg;
           std::vector<yd_task_req> r(N);
           if (reqs) memcpy(r.data(), reqs, size_t(N) * sizeof(yd_task_req));
           else if (reqs16) for (uint32_t i = 0; i != N; ++i) r[i] = yd_unpack_req(reqs16[i]);
@@ -1735,32 +1712,15 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
           s->stats.decisions = N;
           return;
         }
-        solver = 1;
+        plan.solver = 1;
       }
       continue;
     }
-    if (variant == 1) s->solo_hint = s->h_meta.as<uint32_t>()[4] == 0;  // back to one launch when nothing is coupled any more
-    if (variant == 2 || variant == 3) {
-      // completed: the kernel's last block has kept the class table (same class set as the previous such solve) or
-      // cleared it, and re-initialised the rest of the scratch
-      if (variant == 2) sig_now = yd_sched::CleanSig{g_buf_generation, s->z_cls_off, s->z_bytes, s->res_words, s->d_zero.p, s->d_res.p};
-      const unsigned long long fp = s->h_fio->classes_fp;
-      if (fp == s->kept_fp) {
-        s->kept_sig = yd_sched::KeptSig{sig_now, s->topo_gen, s->cls_bound};
-        s->kept_valid = true;
-      } else {
-        s->clean_sig = sig_now;
-        s->clean_valid = true;
-      }
-      s->kept_fp = fp;
-    }  // (variant 4 completed: the kept table stays valid)
-    if (variant == 4) spec = 1;
+    if (plan.variant == kSoloSpec) spec = 1;
     break;
   }
   const Counters* c = s->h_counters.as<Counters>();
   s->next_id += c->granted;
-  s->merge_rounds = merge_rounds_cfg;
-  s->force_stream = force_stream_cfg;
 
   yd_solve_stats& stt = s->stats;
   stt = yd_solve_stats{};
@@ -1769,7 +1729,7 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
   stt.decisions = N;
   stt.granted = c->granted;
   stt.kernel_launches = launches;
-  stt.solver = solver;
+  stt.solver = plan.solver;
   stt.h2d_bytes = (reqs ? size_t(N) * sizeof(yd_task_req) : reqs16 ? size_t(N) * sizeof(yd_task_req16) : 0) + sizeof(yd::DynParams);
   stt.d2h_bytes = size_t(N) * (out8 ? sizeof(yd_grant8) : sizeof(yd_grant)) + sizeof(Counters) + 32;
   s->have_stats = true;
@@ -1783,11 +1743,12 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
     // 1 = k_final_fused, 3 = k_final_count / k_final_scan / k_final_write; `spec` over all attempts; the lease ring
     // (`ring_lo` = the first live id) as the solve found it
     const bool have_work = S && s->n_comps;
-    const uint32_t final_path = (variant >= 2 && have_work && solver == 2) ? 0u : (solver == 2 && have_work && nb <= 2048) ? 1u : 3u;
+    const uint32_t solver = plan.solver;
+    const uint32_t final_path = (IsSolo(plan.variant) && have_work && solver == 2) ? 0u : (solver == 2 && have_work && nb <= 2048) ? 1u : 3u;
     fprintf(stderr, "ydsched: solve n %u tiny 0 variant %u order_static %d wide %d Nb %u slot_b %zu cls_bound %u final %u "
             "emask %d max_comp %zu solver %u graph %d merge_rounds %llu merge_chunks %llu walks %llu windows %llu "
             "spec %u ring_cap %llu ring_lo %llu solve_ms %.3f\n",
-            N, variant, (int)(solver == 2 && s->order_static), (int)s->wide, Nb, slot_b, s->cls_bound, final_path,
+            N, (unsigned)plan.variant, (int)(solver == 2 && s->order_static), (int)s->wide, Nb, slot_b, s->cls_bound, final_path,
             (int)s->emask_ok, (size_t)s->max_comp_servants, solver, (int)graphed, c->pad[0], c->pad[1], c->pad[2],
             c->pad[3], spec, (unsigned long long)s->ring_cap, (unsigned long long)s->lo, stt.solve_ms);
   }

@@ -283,7 +283,7 @@ struct yd_sched {
   uint32_t fused_max_nb = 262144;  // largest batch size class that takes it (YDSCHED_FUSED_MAX_N)
   size_t z_fbar_off = 0;
   DevBuf d_reqs16, d_out8;     // packed upload / download (yd_task_req16, yd_grant8)
-  yd::FusedHostIO* h_fio = nullptr;  // mapped pinned record: the solo kernel's result (no copy nodes after it)
+  yd::FusedHostIO* h_fio = nullptr;  // mapped pinned record: the solo kernel's result (no copy after its launch)
   yd::FusedHostIO* d_fio = nullptr;  // its device-side address
   yd::FusedScalars fsc{};            // the call's scalars: kernel parameters of a solo launch ...
   PinBuf h_fsc;                      // ... or (graphed general sequence) copied into d_fsc by the graph's first node
@@ -331,16 +331,7 @@ struct yd_sched {
     GraphKey key;
     cudaGraphExec_t exec = nullptr;
     uint32_t launches = 0;
-    // solo graphs (one kernel node): the per-call scalars are kernel parameters, patched before every launch
-    cudaGraph_t graph = nullptr;
-    cudaGraphNode_t knode = nullptr;
-    yd::FusedArgs fargs{};
-    uint32_t fgrid = 0;
-    size_t fdyn = 0;
   };
-  yd::FusedArgs last_fused{};  // what LaunchFused passed last (picked up right after a capture)
-  uint32_t last_fused_grid = 0;
-  size_t last_fused_dyn = 0;
   bool host_prof = false;      // YDSCHED_HOST_PROF: host-side timestamps of a solve, printed
   std::vector<GraphEntry> graphs;
   unsigned long long topo_gen = 0;
@@ -365,7 +356,7 @@ struct yd_sched {
   cudaEvent_t ev[6] = {};
   yd_solve_stats stats{};
   bool have_stats = false;
-  int stats_times_pending = 0;  // 1: events of an eager solve, 2: of a graphed one, not yet turned into milliseconds
+  int stats_times_pending = 0;  // 1: events of an eager general solve, 2: of a graphed or solo one, not yet turned into milliseconds
   size_t static_bound_cache = 0;  // StaticSlotBound() of the current facts
 
   yd::ServantArrays arrays() const {
@@ -689,6 +680,8 @@ yd_sched* yd_create(const yd_config* cfg) {
   YD_CUDA_CHECK(cudaEventCreateWithFlags(&s->ev_fork, cudaEventDisableTiming));
   YD_CUDA_CHECK(cudaEventCreateWithFlags(&s->ev_join, cudaEventDisableTiming));
   YD_CUDA_CHECK(cudaEventCreateWithFlags(&s->ev_h2d, cudaEventDisableTiming));
+  // (recorded again only after a request copy; the general graphs' wait nodes name it from their first capture on)
+  YD_CUDA_CHECK(cudaEventRecord(s->ev_h2d, s->st_copy));
   YD_CUDA_CHECK(cudaEventCreateWithFlags(&s->ev_fin, cudaEventDisableTiming));
   s->ips.emplace_back();  // id 0 == YD_IP_NONE == the empty requestor string
   s->ip_ids.emplace("", 0);
@@ -726,7 +719,7 @@ void yd_destroy(yd_sched* s) {
                     &s->d_rt_slots, &s->d_rt_keys, &s->d_rt_out}) {
     b->release();
   }
-  for (auto& g : s->graphs) { if (g.exec) cudaGraphExecDestroy(g.exec); if (g.graph) cudaGraphDestroy(g.graph); }
+  for (auto& g : s->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
   if (s->h_fio) cudaFreeHost(s->h_fio);
   s->d_dyn.release();
   s->d_fsc.release();
@@ -1119,12 +1112,18 @@ uint32_t LaunchCoupledSolvers(yd_sched* s, uint32_t N, size_t slot_b, const Solv
   return launches;
 }
 
+// `st` waits for the request upload on the copy stream: when this call copied requests (`copied`), and always in a
+// capture, whose graph is replayed by calls that copy and calls that do not.  A staged or zero-copy solve outside a graph
+// has nothing to wait for.  `capturing` selects the external-event flavour (the upload is never part of a graph).
+void WaitUpload(yd_sched* s, cudaStream_t st, bool copied, bool capturing) {
+  if (copied || capturing) YD_CUDA_CHECK(cudaStreamWaitEvent(st, s->ev_h2d, capturing ? cudaEventWaitExternal : 0));
+}
+
 // Solver 2: sorted slot streams.  Two concurrent branches:
 //   st  : slot table (+ first histogram) -> radix passes
 //   st2 : [wait for the request upload] class table -> finalize -> FIFO ranks -> scan
-// joined before the per-class lists.  `capturing` selects the external-event flavour of
-// the wait on the upload (the upload itself is never part of the graph).
-uint32_t LaunchStream(yd_sched* s, uint32_t N, size_t slot_b, const SolvePlan& plan, bool capturing) {
+// joined before the per-class lists.
+uint32_t LaunchStream(yd_sched* s, uint32_t N, size_t slot_b, const SolvePlan& plan, bool copied, bool capturing) {
   cudaStream_t st = s->st, st2 = s->st2;
   uint32_t launches = 0;
   yd::TopoView t = MakeTopo(s);
@@ -1139,7 +1138,7 @@ uint32_t LaunchStream(yd_sched* s, uint32_t N, size_t slot_b, const SolvePlan& p
   YD_CUDA_CHECK(cudaEventRecord(s->ev_fork, st));
   YD_CUDA_CHECK(cudaStreamWaitEvent(st2, s->ev_fork, 0));
   // branch B: classes and FIFO ranks (needs the requests in HBM)
-  YD_CUDA_CHECK(cudaStreamWaitEvent(st2, s->ev_h2d, capturing ? cudaEventWaitExternal : 0));
+  WaitUpload(s, st2, copied, capturing);
   yd::k_cls_insert<<<(N + 255) / 256, 256, 0, st2>>>(s->d_reqs.as<yd_task_req>(), dp, t, ct);
   yd::k_cls_finalize<<<1, 1024, 0, st2>>>(t, ct, arr, s->n_comps, s->d_comp_mode.as<uint32_t>());
   YD_CUDA_CHECK(cudaEventRecord(s->ev_fin, st2));  // the list kernels on `st` need the class table, not what follows
@@ -1195,20 +1194,17 @@ uint32_t FusedLoffWords(const yd_sched* s, size_t slot_b) {
   return cells <= 16384 ? (uint32_t)cells : 0u;
 }
 
-// The fused front (fused.cuh): classes, ranks, lists and the data-parallel verdicts in ONE persistent launch on `st`;
-// solo variants: grants, task ids and leases too (batches made of data-parallel components only), else the coupled
-// solvers follow.  Needs the kept slot order.
-uint32_t LaunchFused(yd_sched* s, uint32_t N, size_t slot_b, const SolvePlan& plan, bool capturing, bool packed_in, bool packed_out) {
+// The arguments of the fused front kernel (fused.cuh) for a batch of size class N.  `capturing` (general variants only):
+// the scalars come through a copy node enqueued here; a solo launch, never graphed, gets them as kernel parameters.
+yd::FusedArgs MakeFusedArgs(yd_sched* s, uint32_t N, size_t slot_b, const SolvePlan& plan, bool capturing, bool packed_in,
+                            bool packed_out) {
   const bool solo = IsSolo(plan.variant);
-  cudaStream_t st = s->st;
-  uint32_t launches = 0;
   const uint32_t n_tiles = (uint32_t)((slot_b + yd::kListTile - 1) / yd::kListTile);
   const uint32_t n_rtiles = (N + yd::kRankTile - 1) / yd::kRankTile;
   yd::FusedArgs a{};
   a.sc = s->fsc;
-  // graphed general sequence: the scalars come through a copy node; a solo graph gets them as (patched) kernel parameters
   a.sc_dev = (capturing && !solo) ? s->d_fsc.as<yd::FusedScalars>() : nullptr;
-  if (a.sc_dev) YD_CUDA_CHECK(cudaMemcpyAsync(s->d_fsc.p, s->h_fsc.p, sizeof(yd::FusedScalars), cudaMemcpyHostToDevice, st));
+  if (a.sc_dev) YD_CUDA_CHECK(cudaMemcpyAsync(s->d_fsc.p, s->h_fsc.p, sizeof(yd::FusedScalars), cudaMemcpyHostToDevice, s->st));
   a.hio = s->d_fio;
   a.dyn_out = solo ? nullptr : s->d_dyn.as<yd::DynParams>();
   a.clean_keys = reinterpret_cast<unsigned long long*>(s->d_res.as<uint32_t>() + s->res_words);
@@ -1249,21 +1245,28 @@ uint32_t LaunchFused(yd_sched* s, uint32_t N, size_t slot_b, const SolvePlan& pl
   a.counters = s->d_counters.as<Counters>();
   a.n_servants = (uint32_t)s->sv.size();
   a.prof = s->fused_prof ? s->d_fused_prof.as<unsigned long long>() : nullptr;
-  YD_CUDA_CHECK(cudaStreamWaitEvent(st, s->ev_h2d, capturing ? cudaEventWaitExternal : 0));
-  const uint32_t grid = s->fused_grid;  // one block per SM, whatever the batch: the phases hand out tiles of two kinds
   a.loff_cache_words = solo ? FusedLoffWords(s, slot_b) : 0u;
-  const size_t dyn = size_t(a.loff_cache_words) * 4;
   a.spec = plan.variant == kSoloSpec ? 1u : 0u;
   a.kept_env = s->d_kept_env.as<uint4>();
   a.kept_sv = s->d_kept_sv.as<uint32_t>();
   a.slot_spos = s->d_slot_spos.as<uint32_t>();
-  yd::k_fused_front<<<grid, 1024, dyn, st>>>(a);
-  s->last_fused = a;
-  s->last_fused_grid = grid;
-  s->last_fused_dyn = dyn;
-  launches += 1;
-  if (!solo) launches += LaunchCoupledSolvers(s, N, slot_b, plan, a.L);
-  return launches;
+  return a;
+}
+
+// The fused front kernel on `st`, one block per SM whatever the batch (the phases hand out tiles of two kinds): classes,
+// ranks, lists and the data-parallel verdicts in ONE persistent launch; solo variants: grants, task ids and leases too
+// (batches made of data-parallel components only).  Needs the kept slot order.
+void LaunchFusedKernel(yd_sched* s, const yd::FusedArgs& a) {
+  yd::k_fused_front<<<s->fused_grid, 1024, size_t(a.loff_cache_words) * 4, s->st>>>(a);
+}
+
+// A general (not solo) fused solve: the fused front kernel, then the coupled solvers.
+uint32_t LaunchFused(yd_sched* s, uint32_t N, size_t slot_b, const SolvePlan& plan, bool copied, bool capturing, bool packed_in,
+                     bool packed_out) {
+  const yd::FusedArgs a = MakeFusedArgs(s, N, slot_b, plan, capturing, packed_in, packed_out);
+  WaitUpload(s, s->st, copied, capturing);
+  LaunchFusedKernel(s, a);
+  return 1 + LaunchCoupledSolvers(s, N, slot_b, plan, a.L);
 }
 
 }  // namespace
@@ -1278,11 +1281,12 @@ uint64_t NextPow2(uint64_t v, uint64_t lo) {
   return r;
 }
 
-// Everything between the request upload and the grant download, for size class
-// (Nb, slot_b): the sequence that is captured into a CUDA graph.
+// Everything between the request upload and the grant download, for size class (Nb, slot_b), of a general (not solo)
+// solve: the sequence that is captured into a CUDA graph.  (A solo solve is one kernel: WaitImpl launches it.)
 // packed bit 0: the upload is 16-byte records in d_reqs16; bit 1: the download is 8-byte grants from d_out8.
-uint32_t EnqueueSolve(yd_sched* s, uint32_t Nb, size_t slot_b, const SolvePlan& plan, bool record_events, bool capturing,
-                      uint32_t packed) {
+// `copied`: this call copied the requests on the copy stream (WaitUpload).
+uint32_t EnqueueSolve(yd_sched* s, uint32_t Nb, size_t slot_b, const SolvePlan& plan, bool record_events, bool copied,
+                      bool capturing, uint32_t packed) {
   cudaStream_t st = s->st;
   const uint32_t S = (uint32_t)s->sv.size();
   const uint32_t solver = plan.solver;
@@ -1292,45 +1296,33 @@ uint32_t EnqueueSolve(yd_sched* s, uint32_t Nb, size_t slot_b, const SolvePlan& 
   uint32_t launches = 0;
   const yd::DynParams* dp = s->d_dyn.as<yd::DynParams>();
   const bool fused = plan.variant != kPipeline && have_work && solver == 2;
-  const bool solo = fused && IsSolo(plan.variant);
-  // (the fused kernel reads the call's scalars from the mapped host record and -- not solo -- stores them in d_dyn itself)
+  // (the fused kernel reads the call's scalars from its parameters or d_fsc and stores them in d_dyn itself)
   if (!fused) YD_CUDA_CHECK(cudaMemcpyAsync(s->d_dyn.p, s->h_dyn.p, sizeof(yd::DynParams), cudaMemcpyHostToDevice, st));
-  if (solo) {
-    // the solo kernel keeps the verdicts in registers: only the class-table keys behind res[] are initialised -- and
-    // not even those when the previous solo solve left the scratch clean
-    if (plan.variant == kSolo) {
-      YD_CUDA_CHECK(cudaMemsetAsync(s->d_res.as<uint32_t>() + s->res_words, 0xFF, yd::kClsTableSize * 8, st));
-      YD_CUDA_CHECK(cudaMemsetAsync(static_cast<char*>(s->d_zero.p) + s->z_cls_off, 0, s->z_bytes - s->z_cls_off, st));
-    }
-  } else {
-    // res[] = kResEnvNotFound, and (slot-stream) the class-table keys behind it = empty
-    YD_CUDA_CHECK(cudaMemsetAsync(s->d_res.p, 0xFF, size_t(Nb) * 4 + (solver == 2 ? yd::kClsTableSize * 8 : 0), st));
-    if (solver == 2 && have_work) YD_CUDA_CHECK(cudaMemsetAsync(s->d_zero.p, 0, s->z_bytes, st));
-  }
+  // res[] = kResEnvNotFound, and (slot-stream) the class-table keys behind it = empty
+  YD_CUDA_CHECK(cudaMemsetAsync(s->d_res.p, 0xFF, size_t(Nb) * 4 + (solver == 2 ? yd::kClsTableSize * 8 : 0), st));
+  if (solver == 2 && have_work) YD_CUDA_CHECK(cudaMemsetAsync(s->d_zero.p, 0, s->z_bytes, st));
   if (record_events) YD_CUDA_CHECK(cudaEventRecord(s->ev[1], st));
   const uint32_t* abort_flag = nullptr;
   if (packed_in && !fused) {
     // 16-byte upload -> the 24-byte queue the pipeline kernels read
-    YD_CUDA_CHECK(cudaStreamWaitEvent(st, s->ev_h2d, capturing ? cudaEventWaitExternal : 0));
+    WaitUpload(s, st, copied, capturing);
     yd::k_unpack_reqs<<<(Nb + 255) / 256, 256, 0, st>>>(s->d_reqs16.as<uint4>(), dp, s->d_reqs.as<yd_task_req>());
     launches += 1;
   }
   if (have_work && solver == 2) {
     if (record_events) YD_CUDA_CHECK(cudaEventRecord(s->ev[2], st));
-    if (fused) launches += LaunchFused(s, Nb, slot_b, plan, capturing, packed_in, packed_out);
-    else launches += LaunchStream(s, Nb, slot_b, plan, capturing);
+    if (fused) launches += LaunchFused(s, Nb, slot_b, plan, copied, capturing, packed_in, packed_out);
+    else launches += LaunchStream(s, Nb, slot_b, plan, copied, capturing);
     abort_flag = MakeClassTable(s, plan).meta + 1;
   } else {
     if (have_work) launches += LaunchSlotTable(s, false);
     if (record_events) YD_CUDA_CHECK(cudaEventRecord(s->ev[2], st));
     // the row-scan kernels read the requests: they were uploaded on the copy stream
-    YD_CUDA_CHECK(cudaStreamWaitEvent(st, s->ev_h2d, capturing ? cudaEventWaitExternal : 0));
+    WaitUpload(s, st, copied, capturing);
     if (have_work) launches += LaunchRowscan(s);
   }
   if (record_events) YD_CUDA_CHECK(cudaEventRecord(s->ev[3], st));
-  if (solo) {
-    // grants, ids and leases were written by the fused kernel
-  } else if (solver == 2 && have_work && nb <= 2048) {
+  if (solver == 2 && have_work && nb <= 2048) {
     // grants, task ids (single-pass scan with look-back), leases, ++running_tasks: one launch (beyond ~2 M requests the
     // look-back chain of 1024-thread blocks is slower than three plain passes)
     unsigned long long* look = reinterpret_cast<unsigned long long*>(static_cast<char*>(s->d_zero.p) + s->z_final_off);
@@ -1350,13 +1342,12 @@ uint32_t EnqueueSolve(yd_sched* s, uint32_t Nb, size_t slot_b, const SolvePlan& 
                                            s->d_ever.as<unsigned long long>());
     launches += 3;
   }
-  if (packed_out && !solo) {
+  if (packed_out) {
     yd::k_pack_grants<<<(Nb + 255) / 256, 256, 0, st>>>(s->d_out.as<uint4>(), dp, s->ring(), s->d_out8.as<uint2>());
     launches += 1;
   }
   YD_CUDA_CHECK(cudaGetLastError());
   if (record_events) YD_CUDA_CHECK(cudaEventRecord(s->ev[4], st));
-  if (solo) return launches;  // the kernel left grant count and flags in the mapped host record
   YD_CUDA_CHECK(cudaMemcpyAsync(s->h_counters.p, s->d_counters.p, sizeof(Counters), cudaMemcpyDeviceToHost, st));
   if (abort_flag) {
     YD_CUDA_CHECK(cudaMemcpyAsync(s->h_meta.p, abort_flag - 1, 32, cudaMemcpyDeviceToHost, st));  // meta[0..7]
@@ -1501,17 +1492,21 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
   hp[1] = hp_now();
   YD_CUDA_CHECK(cudaEventRecord(s->ev[0], st));
   // The request upload runs on its own stream so that the slot table and its sort (which
-  // do not read the requests) overlap it; consumers wait on ev_h2d.
+  // do not read the requests) overlap it; consumers wait on ev_h2d, recorded after the copy.
   // (Page-locked caller arrays -- yd_alloc_host -- are not copied at all when the fused kernel runs: its first phase
-  // reads the requests over PCIe itself and, solo, its last phase writes the grants straight into the caller's array.)
-  bool uploaded = false;
+  // reads the requests over PCIe itself and, solo, its last phase writes the grants straight into the caller's array.
+  // Staged requests are in HBM already.  Neither waits for the copy stream.)
+  bool uploaded = false, copied = false;
   auto upload = [&]() {
     if (uploaded) return;
     if (reqs) {
       YD_CUDA_CHECK(cudaMemcpyAsync(s->d_reqs.p, reqs, size_t(N) * sizeof(yd_task_req), cudaMemcpyHostToDevice, s->st_copy));
+      copied = true;
     } else if (reqs16) {
       YD_CUDA_CHECK(cudaMemcpyAsync(s->d_reqs16.p, reqs16, size_t(N) * sizeof(yd_task_req16), cudaMemcpyHostToDevice, s->st_copy));
+      copied = true;
     }
+    if (copied) YD_CUDA_CHECK(cudaEventRecord(s->ev_h2d, s->st_copy));
     uploaded = true;
   };
   auto mapped_address = [&](const void* p) -> void* {
@@ -1555,7 +1550,6 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
     const bool zc_in = plan.variant != kPipeline && in_dev, zc_out = solo && out_dev && in_host;
     hp[2] = hp_now();
     if (!zc_in) upload();
-    YD_CUDA_CHECK(cudaEventRecord(s->ev_h2d, s->st_copy));
     s->fsc.zc_in = zc_in ? in_dev : nullptr;
     s->fsc.zc_out = zc_out ? out_dev : nullptr;
     s->fsc.seq += 1;
@@ -1567,7 +1561,26 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
     if (plan.solver == 2 && want_static && S && s->n_comps && (s->order_dirty || !s->order_static || s->order_slot_b != slot_b)) {
       launches += RebuildSlotOrder(s, slot_b);
     }
-    if (s->use_graphs) {
+    if (solo) {
+      // ONE kernel whose per-call scalars are kernel parameters: launched directly, as a graph would add a parameter
+      // patch and a graph launch to the call.  Its arguments are built before the events, which bracket what the solve
+      // enqueues on `st`; the kernel leaves grant count and flags in the mapped host record.
+      const yd::FusedArgs a = MakeFusedArgs(s, Nb, slot_b, plan, false, packed & 1u, packed & 2u);
+      hp[3] = hp_now();
+      YD_CUDA_CHECK(cudaEventRecord(s->ev[1], st));
+      if (plan.variant == kSolo) {
+        // the solo kernel keeps the verdicts in registers: only the class-table keys behind res[] are initialised --
+        // and not even those when the previous solo solve left the scratch clean (kSoloClean, kSoloSpec)
+        YD_CUDA_CHECK(cudaMemsetAsync(s->d_res.as<uint32_t>() + s->res_words, 0xFF, yd::kClsTableSize * 8, st));
+        YD_CUDA_CHECK(cudaMemsetAsync(static_cast<char*>(s->d_zero.p) + s->z_cls_off, 0, s->z_bytes - s->z_cls_off, st));
+      }
+      WaitUpload(s, st, copied, false);
+      LaunchFusedKernel(s, a);
+      YD_CUDA_CHECK(cudaEventRecord(s->ev[4], st));
+      hp[4] = hp_now();
+      YD_CUDA_CHECK(cudaGetLastError());
+      launches += 1;
+    } else if (s->use_graphs) {
       yd_sched::GraphKey key;
       key.Nb = Nb; key.S = S; key.n_comps = s->n_comps; key.max_comp = s->max_comp_servants;
       key.cls_bound = s->cls_bound; key.solver = plan.solver; key.wide = s->wide; key.slot_b = slot_b;
@@ -1580,50 +1593,17 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
       if (!hit) {
         cudaGraph_t graph = nullptr;
         YD_CUDA_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-        uint32_t l = EnqueueSolve(s, Nb, slot_b, plan, false, true, packed);
+        uint32_t l = EnqueueSolve(s, Nb, slot_b, plan, false, copied, true, packed);
         YD_CUDA_CHECK(cudaStreamEndCapture(st, &graph));
         cudaGraphExec_t exec = nullptr;
         YD_CUDA_CHECK(cudaGraphInstantiate(&exec, graph, 0));
-        yd_sched::GraphEntry ge;
-        ge.key = key; ge.exec = exec; ge.launches = l;
-        if (solo) {
-          // keep the graph: its kernel node is the handle through which the scalars are patched
-          size_t nn = 0;
-          YD_CUDA_CHECK(cudaGraphGetNodes(graph, nullptr, &nn));
-          std::vector<cudaGraphNode_t> nodes(nn);
-          YD_CUDA_CHECK(cudaGraphGetNodes(graph, nodes.data(), &nn));
-          for (cudaGraphNode_t nd : nodes) {
-            cudaGraphNodeType ty;
-            YD_CUDA_CHECK(cudaGraphNodeGetType(nd, &ty));
-            if (ty == cudaGraphNodeTypeKernel) ge.knode = nd;
-          }
-          if (!ge.knode) { fprintf(stderr, "ydsched: no kernel node in the solo graph\n"); abort(); }
-          ge.graph = graph;
-          ge.fargs = s->last_fused;
-          ge.fgrid = s->last_fused_grid;
-          ge.fdyn = s->last_fused_dyn;
-        } else {
-          YD_CUDA_CHECK(cudaGraphDestroy(graph));
-        }
+        YD_CUDA_CHECK(cudaGraphDestroy(graph));
         if (s->graphs.size() >= 16) {  // drop the oldest size class
           cudaGraphExecDestroy(s->graphs.front().exec);
-          if (s->graphs.front().graph) cudaGraphDestroy(s->graphs.front().graph);
           s->graphs.erase(s->graphs.begin());
         }
-        s->graphs.push_back(ge);
+        s->graphs.push_back(yd_sched::GraphEntry{key, exec, l});
         hit = &s->graphs.back();
-      }
-      if (solo) {  // this call's scalars -> the kernel node's parameters
-        hit->fargs.sc = s->fsc;
-        void* kp[1] = {&hit->fargs};
-        cudaKernelNodeParams np{};
-        np.func = reinterpret_cast<void*>(yd::k_fused_front);
-        np.gridDim = dim3(hit->fgrid);
-        np.blockDim = dim3(1024);
-        np.sharedMemBytes = (unsigned)hit->fdyn;
-        np.kernelParams = kp;
-        np.extra = nullptr;
-        YD_CUDA_CHECK(cudaGraphExecKernelNodeSetParams(hit->exec, hit->knode, &np));
       }
       hp[3] = hp_now();
       YD_CUDA_CHECK(cudaEventRecord(s->ev[1], st));
@@ -1633,7 +1613,7 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
       launches += hit->launches;
       graphed = true;
     } else {
-      launches += EnqueueSolve(s, Nb, slot_b, plan, true, false, packed);
+      launches += EnqueueSolve(s, Nb, slot_b, plan, true, copied, false, packed);
     }
     if (plan.solver == 1) { s->order_dirty = true; s->order_static = false; }  // the row-scan solver's table overwrote the kept one
     if (zc_out) {}  // the kernel wrote the grants into the caller's page-locked array
@@ -1643,7 +1623,7 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
     hp[5] = hp_now();
     YD_CUDA_CHECK(cudaStreamSynchronize(st));
     hp[6] = hp_now();
-    if (solo) {  // the solo kernel's report: flags and grant count (there are no copy nodes in its graph)
+    if (solo) {  // the solo kernel's report: flags and grant count (no copy follows its launch)
       if (s->h_fio->done_seq != s->fsc.seq) { fprintf(stderr, "ydsched: the fused kernel left no report\n"); abort(); }
       memcpy(s->h_meta.p, const_cast<const uint32_t*>(s->h_fio->meta), 32);
       s->h_counters.as<Counters>()->granted = s->h_fio->granted;
@@ -1658,7 +1638,7 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
                 t[1] - t[0], t[2] - t[1], t[7] - t[2], t[7] - t[0], (long long)(t[8] - t[7]));
       }
       // every block's stamps (fused.cuh: kProfBlockWords), for tools/dev/phase_prof.py
-      const uint32_t G = s->last_fused_grid;
+      const uint32_t G = s->fused_grid;
       std::vector<unsigned long long> b(size_t(G) * yd::kProfBlockWords);
       YD_CUDA_CHECK(cudaMemcpy(b.data(), s->d_fused_prof.as<unsigned long long>() + yd::kProfHead, b.size() * 8,
                                cudaMemcpyDeviceToHost));
@@ -1725,7 +1705,7 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
   yd_solve_stats& stt = s->stats;
   stt = yd_solve_stats{};
   // (the event arithmetic costs a driver call apiece: done when yd_last_solve_stats asks, the events stay valid until the next solve)
-  s->stats_times_pending = graphed ? 2 : 1;
+  s->stats_times_pending = (graphed || IsSolo(plan.variant)) ? 2 : 1;
   stt.decisions = N;
   stt.granted = c->granted;
   stt.kernel_launches = launches;
@@ -1735,7 +1715,7 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
   s->have_stats = true;
   if (s->host_prof) {
     hp[7] = hp_now();
-    fprintf(stderr, "ydsched: host us: prep %.1f (attrs+variant %.1f) upload+event+setparams %.1f launch %.1f d2h-enqueue %.1f sync-wait %.1f stats %.1f total %.1f\n",
+    fprintf(stderr, "ydsched: host us: prep %.1f (attrs+variant %.1f) upload+prep %.1f launch %.1f d2h-enqueue %.1f sync-wait %.1f stats %.1f total %.1f\n",
             hp[1] - hp[0], hp[2] - hp[1], hp[3] - hp[2], hp[4] - hp[3], hp[5] - hp[4], hp[6] - hp[5], hp[7] - hp[6], hp[7] - hp[0]);
   }
   if (s->debug_env) {
@@ -2054,7 +2034,7 @@ int yd_last_solve_stats(yd_sched* s, yd_solve_stats* out) {
     yd_solve_stats& stt = s->stats;
     cudaEventElapsedTime(&ms, s->ev[0], s->ev[5]); stt.total_ms = ms;
     if (s->stats_times_pending == 2) {
-      // inside a graph the phases are not separable: solve_ms is the whole device pipeline
+      // inside a graph, or around the one solo launch, the phases are not separable: solve_ms is the whole device pipeline
       cudaEventElapsedTime(&ms, s->ev[1], s->ev[4]); stt.solve_ms = ms;
     } else {
       cudaEventElapsedTime(&ms, s->ev[1], s->ev[2]); stt.prep_ms = ms;

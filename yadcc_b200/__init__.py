@@ -27,4 +27,5 @@ from ._abi import (  # noqa: F401
     cuda_library_path,
     load_library,
 )
-from .dispatcher import Servant, RunningTask, TaskAllocation, TaskDispatcher, WaitStatus, pack_requests, unpack_grants  # noqa: F401
+from .dispatcher import (Servant, RunningTask, TaskAllocation, TaskDispatcher, TaskKeysError, TaskSources, WaitStatus,  # noqa: F401
+                         pack_requests, unpack_grants)

@@ -71,6 +71,17 @@ class yd_prefilter(C.Structure):
 FILTER_OFFERED, FILTER_CACHE_HIT, FILTER_JOINED = 0, 1, 2
 
 
+class yd_task_sources(C.Structure):
+    _fields_ = [("args", C.c_void_p), ("args_offsets", C.c_void_p), ("n_args", C.c_size_t), ("args_index", C.c_void_p),
+                ("source_digests", C.c_void_p), ("source_digest_len", C.c_size_t), ("source_digest_stride", C.c_size_t)]
+
+
+KEYS_OK, KEYS_BAD_SOURCES, KEYS_UNKNOWN_ENV, KEYS_BAD_ARGS_INDEX, KEYS_TOO_LONG = 0, 1, 2, 3, 4
+KEYS_CACHE_KEY_LEN, KEYS_TASK_DIGEST_LEN = 81, 64
+KEYS_MAX_ARGS_LEN, KEYS_MAX_DIGEST_LEN = 256 << 10, 64 << 10
+STAGE_CACHE, STAGE_DEDUPE = 1, 2
+
+
 class yd_config(C.Structure):
     _fields_ = [
         ("abi_version", C.c_uint32),
@@ -259,8 +270,9 @@ def load_library(path: os.PathLike | str | None = None) -> C.CDLL:
         fn = getattr(lib, name)  # AttributeError if the symbol is missing
         fn.restype = restype
         fn.argtypes = argtypes
-    # include/ydstate.h: the CUDA library and the port's state build (checkers/) export and import state
-    for name, restype, argtypes in STATE_PROTOTYPES:
+    # include/ydstate.h: the CUDA library and the port's state build (checkers/) export and import state; the task keys
+    # are exported by the CUDA library and the checkers' key builds
+    for name, restype, argtypes in STATE_PROTOTYPES + KEYS_PROTOTYPES:
         fn = getattr(lib, name, None)
         if fn is not None:
             fn.restype = restype
@@ -300,6 +312,13 @@ SHARD_PROTOTYPES = [
 ]
 
 # Every symbol include/ydstate.h declares, and its status codes.
+# include/ydkeys.h: the task keys, exported by the CUDA library and by the checkers' builds that have them
+KEYS_PROTOTYPES = [
+    ("yd_derive_task_keys", C.c_int, [_P, _P, C.c_size_t, _P, _P, _P]),
+    ("yd_derive_filter_and_wait_for_starting_new_tasks", C.c_size_t,
+     [_P, C.c_int64, _P, C.c_size_t, _P, C.c_uint32, _P, _P, _P]),
+]
+
 STATE_PROTOTYPES = [
     ("yd_export_state", C.c_size_t, [_P, C.c_int64, _P, C.c_size_t]),
     ("yd_import_state", C.c_int, [_P, C.c_int64, _P, C.c_size_t]),

@@ -18,6 +18,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <numeric>
+#include <type_traits>
 #include <string>
 #include <unordered_map>
 #include <vector>
@@ -35,8 +36,11 @@
 #include "tiny.cuh"
 #include "fused.cuh"
 #include "filter.cuh"
+#include "blake3.cuh"
 #include "state.cuh"
 #include "ydstate_codec.inc"
+#include "ydkeys.h"
+#include "ydsched_keys_impl.inc"
 
 namespace {
 
@@ -350,6 +354,11 @@ struct yd_sched {
   DevBuf d_freqs, d_fverdict, d_ftile;  // pre-filtered solve (filter.cuh): the unfiltered queue, verdicts, tile counts
   PinBuf h_fcount;
   cudaEvent_t ev_f[2] = {};
+  // the env table on the device (blake3.cuh): digest e = env_bytes[env_off[e] .. env_off[e + 1]) for e < env_dev_n,
+  // appended from `envs` before a derivation reads it.  Allocated stream-ordered, outside the grow-only buffers.
+  unsigned char* d_env_bytes = nullptr;
+  uint32_t* d_env_off = nullptr;
+  size_t env_dev_n = 0, env_dev_bytes = 0, env_cap_n = 0, env_cap_bytes = 0;
   uint32_t rt_mask = 0;
   size_t rt_distinct = 0;
 
@@ -727,6 +736,8 @@ void yd_destroy(yd_sched* s) {
   for (auto& e : s->ev) cudaEventDestroy(e);
   for (auto& e : s->ev_f) cudaEventDestroy(e);
   for (DevBuf* b : {&s->d_freqs, &s->d_fverdict, &s->d_ftile}) b->release();
+  if (s->d_env_bytes) cudaFree(s->d_env_bytes);
+  if (s->d_env_off) cudaFree(s->d_env_off);
   s->h_fcount.release();
   cudaEventDestroy(s->ev_fork); cudaEventDestroy(s->ev_join); cudaEventDestroy(s->ev_h2d); cudaEventDestroy(s->ev_fin);
   cudaStreamDestroy(s->st2); cudaStreamDestroy(s->st_copy);
@@ -2231,51 +2242,42 @@ int yd_running_index_entry(yd_sched* s, uint32_t i, yd_running_task* out) {
   return 1;
 }
 
-// BASELINE configs[3] in one call: bloom probes, in-flight index probes, order-preserving compaction and the solve,
-// with the queue resident in HBM from the first stage to the last (filter.cuh).
-size_t yd_filter_and_wait_for_starting_new_tasks(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, size_t n,
-                                                 const yd_prefilter* f, uint8_t* verdict_out, yd_running_hit* hits_out,
-                                                 yd_grant* grants_out) {
-  if (n == 0) return 0;
-  if (n > 0x40000000ull) { fprintf(stderr, "ydsched: batch too large\n"); abort(); }
-  YD_CUDA_CHECK(cudaSetDevice(s->device));
-  cudaStream_t st = s->st;
-  const uint32_t N = (uint32_t)n;
+// The pre-filtered solve's buffers for a queue of N requests, cache keys (key_span bytes) if `bloom`, task digests
+// (digest_span bytes) if `dedupe`.  Drops the staged queue.
+static void FilterPrepare(yd_sched* s, uint32_t N, bool bloom, size_t key_span, bool dedupe, size_t digest_span) {
   const uint32_t nt = (N + 1023) / 1024;
-  const bool bloom = f && f->cache_keys, dedupe = f && f->task_digests;
-  if (bloom) {
-    if (!s->bloom_bits) { fprintf(stderr, "ydsched: bloom filter used before yd_bloom_reset / yd_bloom_load\n"); abort(); }
-    if (f->cache_key_len > yd::kBloomMaxKey) { fprintf(stderr, "ydsched: bloom keys longer than %d bytes\n", yd::kBloomMaxKey); abort(); }
-  }
   s->d_freqs.ensure(size_t(N) * sizeof(yd_task_req));
   s->d_fverdict.ensure(N);
   s->d_ftile.ensure(size_t(nt + 1) * 4);
   s->d_reqs.ensure(size_t(NextPow2(N, 1024)) * sizeof(yd_task_req));
   s->h_fcount.ensure(16);
   s->staged_n = 0;
-  // uploads: the queue, the cache keys, the task digests (one stream: each stage starts when its input has landed)
-  YD_CUDA_CHECK(cudaMemcpyAsync(s->d_freqs.p, reqs, size_t(N) * sizeof(yd_task_req), cudaMemcpyHostToDevice, st));
   if (bloom) {
-    const size_t span = (n - 1) * f->cache_key_stride + f->cache_key_len;
-    s->d_bloom_keys.ensure(span ? span : 1);
-    s->d_bloom_out.ensure(n);
-    YD_CUDA_CHECK(cudaMemcpyAsync(s->d_bloom_keys.p, f->cache_keys, span, cudaMemcpyHostToDevice, st));
+    s->d_bloom_keys.ensure(key_span ? key_span : 1);
+    s->d_bloom_out.ensure(N);
   }
   if (dedupe) {
-    const size_t span = (n - 1) * f->task_digest_stride + f->task_digest_len;
-    s->d_rt_keys.ensure(span ? span : 1);
-    s->d_rt_out.ensure(n * sizeof(yd_running_hit));
-    YD_CUDA_CHECK(cudaMemcpyAsync(s->d_rt_keys.p, f->task_digests, span, cudaMemcpyHostToDevice, st));
+    s->d_rt_keys.ensure(digest_span ? digest_span : 1);
+    s->d_rt_out.ensure(size_t(N) * sizeof(yd_running_hit));
   }
-  YD_CUDA_CHECK(cudaEventRecord(s->ev_f[0], st));
+}
+
+// The device part of the pre-filtered solve, from the first filter stage on: the queue is in d_freqs, the cache keys
+// (if `bloom`) in d_bloom_keys, the task digests (if `dedupe`) in d_rt_keys, and ev_f[0] has been recorded.
+static size_t FilterStages(yd_sched* s, int64_t now_ns, uint32_t N, bool bloom, size_t key_len, size_t key_stride, bool dedupe,
+                           size_t digest_len, size_t digest_stride, uint8_t* verdict_out, yd_running_hit* hits_out,
+                           yd_grant* grants_out, size_t h2d_bytes, uint32_t extra_launches) {
+  cudaStream_t st = s->st;
+  const size_t n = N;
+  const uint32_t nt = (N + 1023) / 1024;
   if (bloom) {
-    yd::k_bloom<false><<<(N + 127) / 128, 128, 0, st>>>(s->d_bloom_keys.as<unsigned char>(), N, (uint32_t)f->cache_key_len,
-                                                        f->cache_key_stride, s->bloom_hashes, s->bloom_bits - 1,
+    yd::k_bloom<false><<<(N + 127) / 128, 128, 0, st>>>(s->d_bloom_keys.as<unsigned char>(), N, (uint32_t)key_len,
+                                                        key_stride, s->bloom_hashes, s->bloom_bits - 1,
                                                         s->d_bloom.as<uint32_t>(), s->d_bloom_out.as<uint8_t>());
   }
   if (dedupe) {
     yd::k_rt_find<<<(N + 255) / 256, 256, 0, st>>>(MakeRtIndex(s), s->d_rt_keys.as<unsigned char>(), N,
-                                                   (uint32_t)f->task_digest_len, f->task_digest_stride,
+                                                   (uint32_t)digest_len, digest_stride,
                                                    s->d_rt_ids.as<unsigned long long>(), s->d_rt_out.as<uint4>());
   }
   yd::k_keep_count<<<nt, 1024, 0, st>>>(bloom ? s->d_bloom_out.as<uint8_t>() : nullptr, dedupe ? s->d_rt_out.as<uint4>() : nullptr, N,
@@ -2308,12 +2310,180 @@ size_t yd_filter_and_wait_for_starting_new_tasks(yd_sched* s, int64_t now_ns, co
   // stats of the whole call: prep = the filter stages + compaction (device), solve / final = the solve's, decisions = n
   s->stats.prep_ms += filter_ms;
   s->stats.decisions = N;
-  s->stats.kernel_launches += 3 + (bloom ? 1 : 0) + (dedupe ? 1 : 0);
-  s->stats.h2d_bytes += size_t(N) * sizeof(yd_task_req) + (bloom ? (n - 1) * f->cache_key_stride + f->cache_key_len : 0) +
-                        (dedupe ? (n - 1) * f->task_digest_stride + f->task_digest_len : 0);
+  s->stats.kernel_launches += 3 + (bloom ? 1 : 0) + (dedupe ? 1 : 0) + extra_launches;
+  s->stats.h2d_bytes += h2d_bytes;
   s->stats.d2h_bytes += N + 4 + (hits_out && dedupe ? n * sizeof(yd_running_hit) : 0);
   return kept;
 }
+
+// BASELINE configs[3] in one call: bloom probes, in-flight index probes, order-preserving compaction and the solve,
+// with the queue resident in HBM from the first stage to the last (filter.cuh).
+size_t yd_filter_and_wait_for_starting_new_tasks(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, size_t n,
+                                                 const yd_prefilter* f, uint8_t* verdict_out, yd_running_hit* hits_out,
+                                                 yd_grant* grants_out) {
+  if (n == 0) return 0;
+  if (n > 0x40000000ull) { fprintf(stderr, "ydsched: batch too large\n"); abort(); }
+  YD_CUDA_CHECK(cudaSetDevice(s->device));
+  cudaStream_t st = s->st;
+  const uint32_t N = (uint32_t)n;
+  const bool bloom = f && f->cache_keys, dedupe = f && f->task_digests;
+  if (bloom) {
+    if (!s->bloom_bits) { fprintf(stderr, "ydsched: bloom filter used before yd_bloom_reset / yd_bloom_load\n"); abort(); }
+    if (f->cache_key_len > yd::kBloomMaxKey) { fprintf(stderr, "ydsched: bloom keys longer than %d bytes\n", yd::kBloomMaxKey); abort(); }
+  }
+  const size_t key_span = bloom ? (n - 1) * f->cache_key_stride + f->cache_key_len : 0;
+  const size_t digest_span = dedupe ? (n - 1) * f->task_digest_stride + f->task_digest_len : 0;
+  FilterPrepare(s, N, bloom, key_span, dedupe, digest_span);
+  // uploads: the queue, the cache keys, the task digests (one stream: each stage starts when its input has landed)
+  YD_CUDA_CHECK(cudaMemcpyAsync(s->d_freqs.p, reqs, size_t(N) * sizeof(yd_task_req), cudaMemcpyHostToDevice, st));
+  if (bloom) YD_CUDA_CHECK(cudaMemcpyAsync(s->d_bloom_keys.p, f->cache_keys, key_span, cudaMemcpyHostToDevice, st));
+  if (dedupe) YD_CUDA_CHECK(cudaMemcpyAsync(s->d_rt_keys.p, f->task_digests, digest_span, cudaMemcpyHostToDevice, st));
+  YD_CUDA_CHECK(cudaEventRecord(s->ev_f[0], st));
+  return FilterStages(s, now_ns, N, bloom, bloom ? f->cache_key_len : 0, bloom ? f->cache_key_stride : 0, dedupe,
+                      dedupe ? f->task_digest_len : 0, dedupe ? f->task_digest_stride : 0, verdict_out, hits_out, grants_out,
+                      size_t(N) * sizeof(yd_task_req) + key_span + digest_span, 0);
+}
+
+// ---- cache keys and task digests from task descriptors (blake3.cuh) ------------------------------------------------
+
+// Appends the digests interned since the last derivation to the device env table (yd_intern_env, heartbeats and
+// yd_import_state all intern through `envs`, which only grows).  Returns the bytes uploaded.
+static size_t SyncEnvTable(yd_sched* s) {
+  const size_t E = s->envs.size();
+  if (E == s->env_dev_n && s->d_env_off) return 0;
+  cudaStream_t st = s->st;
+  std::vector<uint32_t> off(E - s->env_dev_n + 1);
+  std::string bytes;
+  off[0] = (uint32_t)s->env_dev_bytes;
+  for (size_t e = s->env_dev_n; e != E; ++e) {
+    bytes += s->envs[e];
+    if (s->env_dev_bytes + bytes.size() > 0xffffff00ull) { fprintf(stderr, "ydsched: interned digests exceed 4 GiB\n"); abort(); }
+    off[e - s->env_dev_n + 1] = (uint32_t)(s->env_dev_bytes + bytes.size());
+  }
+  // grown by doubling, stream-ordered; the old contents are copied over
+  auto grow = [&](auto*& p, size_t used, size_t need, size_t& cap) {
+    if (need <= cap && p) return;
+    size_t ncap = std::max<size_t>(std::max(need, cap * 2), 256);
+    void* np = nullptr;
+    YD_CUDA_CHECK(cudaMallocAsync(&np, ncap + 8, st));  // + 8: LoadU32 reads whole aligned words
+    if (p) {
+      if (used) YD_CUDA_CHECK(cudaMemcpyAsync(np, p, used, cudaMemcpyDeviceToDevice, st));
+      YD_CUDA_CHECK(cudaFreeAsync(p, st));
+    }
+    p = static_cast<std::remove_reference_t<decltype(p)>>(np);
+    cap = ncap;
+  };
+  grow(s->d_env_bytes, s->env_dev_bytes, s->env_dev_bytes + bytes.size(), s->env_cap_bytes);
+  grow(s->d_env_off, (s->env_dev_n + 1) * 4, (E + 1) * 4, s->env_cap_n);
+  if (!bytes.empty())
+    YD_CUDA_CHECK(cudaMemcpyAsync(s->d_env_bytes + s->env_dev_bytes, bytes.data(), bytes.size(), cudaMemcpyHostToDevice, st));
+  YD_CUDA_CHECK(cudaMemcpyAsync(s->d_env_off + s->env_dev_n, off.data(), off.size() * 4, cudaMemcpyHostToDevice, st));
+  YD_CUDA_CHECK(cudaStreamSynchronize(st));  // (the staging strings go out of scope)
+  s->env_dev_n = E;
+  s->env_dev_bytes += bytes.size();
+  return bytes.size() + off.size() * 4;
+}
+
+// The per-call descriptors on the device, in one stream-ordered scratch allocation (StateTmp's discipline: the
+// grow-only buffers, whose reallocation drops the kept class table, are not touched).  `reqs_dev` is where the kernel
+// reads the requests' env ids; null: they are uploaded into the scratch too.
+struct KeyScratch {
+  void* base = nullptr;
+  size_t h2d = 0;
+  yd::KeySources ks{};
+};
+
+static KeyScratch UploadKeySources(yd_sched* s, const yd_task_req* reqs, const yd_task_req* reqs_dev, size_t n,
+                                   const yd_task_sources* src, size_t out_bytes) {
+  cudaStream_t st = s->st;
+  KeyScratch k;
+  k.h2d = SyncEnvTable(s);
+  auto al = [](size_t b) { return (b + 15) & ~size_t(15); };
+  const size_t args_b = src->args_offsets[src->n_args], off_b = (src->n_args + 1) * 8, idx_b = n * 4;
+  const size_t sd_b = src->source_digest_len ? (n - 1) * src->source_digest_stride + src->source_digest_len : 0;
+  const size_t req_b = reqs_dev ? 0 : n * sizeof(yd_task_req);
+  const size_t total = al(args_b + 8) + al(off_b) + al(idx_b) + al(sd_b + 8) + al(req_b) + out_bytes;
+  YD_CUDA_CHECK(cudaMallocAsync(&k.base, total, st));
+  char* p = static_cast<char*>(k.base);
+  auto put = [&](const void* h, size_t b, size_t room) {
+    if (b) YD_CUDA_CHECK(cudaMemcpyAsync(p, h, b, cudaMemcpyHostToDevice, st));
+    k.h2d += b;
+    char* at = p;
+    p += al(room);
+    return at;
+  };
+  k.ks.args = reinterpret_cast<const unsigned char*>(put(src->args, args_b, args_b + 8));
+  k.ks.args_off = reinterpret_cast<const unsigned long long*>(put(src->args_offsets, off_b, off_b));
+  k.ks.args_index = reinterpret_cast<const uint32_t*>(put(src->args_index, idx_b, idx_b));
+  k.ks.src = reinterpret_cast<const unsigned char*>(put(src->source_digests, sd_b, sd_b + 8));
+  k.ks.reqs = reqs_dev ? reqs_dev : reinterpret_cast<const yd_task_req*>(put(reqs, req_b, req_b));
+  k.ks.src_stride = src->source_digest_stride;
+  k.ks.src_len = (uint32_t)src->source_digest_len;
+  k.ks.env_bytes = s->d_env_bytes;
+  k.ks.env_off = s->d_env_off;
+  k.ks.n = (uint32_t)n;
+  k.ks.cache_keys = reinterpret_cast<unsigned char*>(p);  // the outputs' room, if any (the caller points them elsewhere)
+  return k;
+}
+
+static void LaunchTaskKeys(yd_sched* s, yd::KeySources ks) {
+  ks.both = ks.cache_keys && ks.task_digests;
+  const size_t threads = size_t(ks.n) << ks.both;
+  yd::k_task_keys<<<(unsigned)((threads + 127) / 128), 128, 0, s->st>>>(ks);
+  YD_CUDA_CHECK(cudaGetLastError());
+}
+
+int yd_derive_task_keys(yd_sched* s, const yd_task_req* reqs, size_t n, const yd_task_sources* src, char* cache_keys_out,
+                        char* task_digests_out) {
+  if (int rc = yd_keys_check(s->envs, reqs, n, src)) return rc;
+  if (n == 0 || (!cache_keys_out && !task_digests_out)) return YD_KEYS_OK;
+  if (n > 0x40000000ull) { fprintf(stderr, "ydsched: batch too large\n"); abort(); }
+  YD_CUDA_CHECK(cudaSetDevice(s->device));
+  cudaStream_t st = s->st;
+  const size_t kb = cache_keys_out ? n * YD_KEYS_CACHE_KEY_LEN : 0, db = task_digests_out ? n * YD_KEYS_TASK_DIGEST_LEN : 0;
+  KeyScratch k = UploadKeySources(s, reqs, nullptr, n, src, kb + db);
+  unsigned char* room = k.ks.cache_keys;
+  k.ks.cache_keys = cache_keys_out ? room : nullptr;
+  k.ks.task_digests = task_digests_out ? room + kb : nullptr;
+  LaunchTaskKeys(s, k.ks);
+  if (cache_keys_out) YD_CUDA_CHECK(cudaMemcpyAsync(cache_keys_out, room, kb, cudaMemcpyDeviceToHost, st));
+  if (task_digests_out) YD_CUDA_CHECK(cudaMemcpyAsync(task_digests_out, room + kb, db, cudaMemcpyDeviceToHost, st));
+  YD_CUDA_CHECK(cudaFreeAsync(k.base, st));
+  YD_CUDA_CHECK(cudaStreamSynchronize(st));
+  return YD_KEYS_OK;
+}
+
+// The pre-filtered solve from descriptors: the keys are derived straight into d_bloom_keys / d_rt_keys, at the strides
+// the filter stages read, so from there on it is yd_filter_and_wait_for_starting_new_tasks' device part unchanged.
+size_t yd_derive_filter_and_wait_for_starting_new_tasks(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, size_t n,
+                                                        const yd_task_sources* src, uint32_t stages, uint8_t* verdict_out,
+                                                        yd_running_hit* hits_out, yd_grant* grants_out) {
+  if (yd_keys_check(s->envs, reqs, n, src) != YD_KEYS_OK) return (size_t)-1;
+  if (n == 0) return 0;
+  if (n > 0x40000000ull) { fprintf(stderr, "ydsched: batch too large\n"); abort(); }
+  const bool bloom = stages & YD_STAGE_CACHE, dedupe = stages & YD_STAGE_DEDUPE;
+  if (bloom && !s->bloom_bits) { fprintf(stderr, "ydsched: bloom filter used before yd_bloom_reset / yd_bloom_load\n"); abort(); }
+  YD_CUDA_CHECK(cudaSetDevice(s->device));
+  cudaStream_t st = s->st;
+  const uint32_t N = (uint32_t)n;
+  FilterPrepare(s, N, bloom, n * YD_KEYS_CACHE_KEY_LEN, dedupe, n * YD_KEYS_TASK_DIGEST_LEN);
+  YD_CUDA_CHECK(cudaMemcpyAsync(s->d_freqs.p, reqs, size_t(N) * sizeof(yd_task_req), cudaMemcpyHostToDevice, st));
+  KeyScratch k{};
+  if (bloom || dedupe) {
+    k = UploadKeySources(s, reqs, s->d_freqs.as<yd_task_req>(), n, src, 0);
+    k.ks.cache_keys = bloom ? s->d_bloom_keys.as<unsigned char>() : nullptr;
+    k.ks.task_digests = dedupe ? s->d_rt_keys.as<unsigned char>() : nullptr;
+  }
+  YD_CUDA_CHECK(cudaEventRecord(s->ev_f[0], st));  // (prep_ms: from the derivation on)
+  if (bloom || dedupe) {
+    LaunchTaskKeys(s, k.ks);
+    YD_CUDA_CHECK(cudaFreeAsync(k.base, st));
+  }
+  return FilterStages(s, now_ns, N, bloom, YD_KEYS_CACHE_KEY_LEN, YD_KEYS_CACHE_KEY_LEN, dedupe, YD_KEYS_TASK_DIGEST_LEN,
+                      YD_KEYS_TASK_DIGEST_LEN, verdict_out, hits_out, grants_out, size_t(N) * sizeof(yd_task_req) + k.h2d,
+                      (bloom || dedupe) ? 1u : 0u);
+}
+
 
 }  // extern "C"
 

@@ -85,6 +85,42 @@ class StateError(RuntimeError):
         self.code = code
 
 
+class TaskKeysError(ValueError):
+    """yd_derive_task_keys refused its input (a YD_KEYS_* code); nothing was written or decided."""
+
+    NAMES = {1: "bad sources", 2: "unknown env id", 3: "argument index out of range", 4: "string too long"}
+
+    def __init__(self, code: int):
+        super().__init__(f"task keys: {self.NAMES.get(code, code)} (code {code})")
+        self.code = code
+
+
+@dataclass
+class TaskSources:
+    """The descriptors yd_derive_task_keys hashes, laid out as yd_task_sources: the call's distinct
+    invocation-argument strings back to back, per request an index into them and a fixed-length source
+    digest.  Build one with ``TaskSources.of`` and reuse it across calls."""
+
+    args: np.ndarray            # uint8, the strings back to back
+    args_offsets: np.ndarray    # uint64[n_args + 1]
+    args_index: np.ndarray      # uint32[n]
+    source_digests: np.ndarray  # uint8[n, source_digest_len]
+
+    @classmethod
+    def of(cls, args: Sequence[str | bytes], args_index, source_digests) -> "TaskSources":
+        b = [a.encode() if isinstance(a, str) else bytes(a) for a in args]
+        off = np.zeros(len(b) + 1, dtype=np.uint64)
+        off[1:] = np.cumsum([len(x) for x in b], dtype=np.uint64)
+        blob = np.frombuffer(b"".join(b) or b"\0", dtype=np.uint8).copy()
+        return cls(blob, off, np.ascontiguousarray(args_index, dtype=np.uint32), TaskDispatcher._key_matrix(source_digests))
+
+    def struct(self) -> "_abi.yd_task_sources":
+        sd = self.source_digests
+        return _abi.yd_task_sources(self.args.ctypes.data, self.args_offsets.ctypes.data, len(self.args_offsets) - 1,
+                                    self.args_index.ctypes.data, sd.ctypes.data if sd.size else None, sd.shape[1],
+                                    sd.strides[0] if sd.shape[1] else 0)
+
+
 def _ns(seconds: float | int) -> int:
     return int(round(seconds * 1_000_000_000))
 
@@ -502,6 +538,47 @@ class TaskDispatcher:
                                                                 out.ctypes.data)
         return verdict, hits, out[: int(k)]
 
+    # -- cache keys and task digests from task descriptors (yd_derive_task_keys) --------------
+    def derive_task_keys(self, reqs: np.ndarray, src: TaskSources, *, cache_keys: bool = True, task_digests: bool = True):
+        """GetCxxCacheEntryKey / GetCxxTaskDigest for every request: ((n, 81) uint8 or None, (n, 64) uint8 or None),
+        ready for bloom_* and find_running_tasks.  Raises TaskKeysError on input the call refuses."""
+        assert reqs.dtype == REQ_DTYPE and reqs.flags.c_contiguous
+        n = reqs.shape[0]
+        assert len(src.args_index) >= n and src.source_digests.shape[0] >= n
+        km = np.zeros((n, _abi.KEYS_CACHE_KEY_LEN), dtype=np.uint8) if cache_keys else None
+        dm = np.zeros((n, _abi.KEYS_TASK_DIGEST_LEN), dtype=np.uint8) if task_digests else None
+        f = src.struct()
+        rc = self._optional_fn("yd_derive_task_keys")(self._h, reqs.ctypes.data, n, C.byref(f), km.ctypes.data if cache_keys else None,
+                                           dm.ctypes.data if task_digests else None)
+        if rc:
+            raise TaskKeysError(rc)
+        return km, dm
+
+    def derive_filter_and_wait_for_starting_new_tasks(self, reqs: np.ndarray, src: TaskSources,
+                                                      stages: int = _abi.STAGE_CACHE | _abi.STAGE_DEDUPE, now: float = 0.0,
+                                                      out: np.ndarray | None = None, verdict_out: np.ndarray | None = None,
+                                                      want_hits: bool = True):
+        """filter_and_wait_for_starting_new_tasks with the cache keys and task digests derived from `src`
+        (yd_derive_filter_and_wait_for_starting_new_tasks): (verdicts, hits, grants of the offered requests).
+        Raises TaskKeysError, deciding nothing, on input the call refuses."""
+        assert reqs.dtype == REQ_DTYPE and reqs.flags.c_contiguous
+        n = reqs.shape[0]
+        assert len(src.args_index) >= n and src.source_digests.shape[0] >= n
+        verdict = verdict_out[:n] if verdict_out is not None else np.zeros(n, dtype=np.uint8)
+        assert verdict.dtype == np.uint8 and verdict.shape[0] == n and verdict.flags.c_contiguous
+        hits = np.zeros(n, dtype=_abi.RUNNING_HIT_DTYPE) if want_hits else None
+        if out is None:
+            out = np.zeros(max(n, 1), dtype=GRANT_DTYPE)
+        assert out.dtype == GRANT_DTYPE and out.shape[0] >= n and out.flags.c_contiguous
+        f = src.struct()
+        k = self._optional_fn("yd_derive_filter_and_wait_for_starting_new_tasks")(
+            self._h, _ns(now), reqs.ctypes.data, n, C.byref(f), int(stages), verdict.ctypes.data,
+            hits.ctypes.data if want_hits else None, out.ctypes.data)
+        if k == C.c_size_t(-1).value:
+            code = self._optional_fn("yd_derive_task_keys")(self._h, reqs.ctypes.data, n, C.byref(f), None, None)
+            raise TaskKeysError(code)
+        return verdict, hits, out[: int(k)]
+
     def running_index_entry(self, snapshot_index: int) -> RunningTask | None:
         t = _abi.yd_running_task()
         import ctypes as C
@@ -511,17 +588,18 @@ class TaskDispatcher:
         return RunningTask(int(t.servant_task_id), int(t.task_grant_id), (t.servant_location or b"").decode(),
                            (t.task_digest or b"").decode())
 
-    # -- state export / import (include/ydstate.h) --------------------------
-    def _state_fn(self, name: str):
+    def _optional_fn(self, name: str):
+        """An entry point not every checker build exports (the state export / import, the task keys)."""
         fn = getattr(self._lib, name, None)
         if fn is None:
             raise NotImplementedError(f"{self._lib._yd_path} does not export {name}")
         return fn
 
+    # -- state export / import (include/ydstate.h) --------------------------
     def export_state(self, now: float = 0.0, *, now_ns: int | None = None) -> bytes:
         """The handle's decision state (servants, leases, next task id, running-task bookkeeping, intern
         tables) in the versioned format of ydstate.h, times relative to `now`."""
-        fn = self._state_fn("yd_export_state")
+        fn = self._optional_fn("yd_export_state")
         t = now_ns if now_ns is not None else _ns(now)
         n = fn(self._h, t, None, 0)
         if n == 0:
@@ -534,7 +612,7 @@ class TaskDispatcher:
     def import_state(self, blob: bytes, now: float = 0.0, *, now_ns: int | None = None) -> None:
         """Load an export into this handle, which must be fresh (no call since construction).  Times are
         rebased onto `now`.  Raises StateError with the ydstate.h status code if the export is refused."""
-        fn = self._state_fn("yd_import_state")
+        fn = self._optional_fn("yd_import_state")
         data = bytes(blob)
         rc = fn(self._h, now_ns if now_ns is not None else _ns(now), data, len(data))
         if rc != _abi.STATE_OK:

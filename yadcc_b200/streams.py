@@ -436,6 +436,31 @@ def config2(n_tasks: int = 100_000, n_servants: int = 2000, n_digests: int = 8, 
                     {"tasks": n_tasks, "servants": n_servants, "digests": n_digests, "variant": variant})
 
 
+def config3_task_sources(n: int = 100_000, seed: int = 47, n_tus: int = 6124, n_args: int = 40) -> "TaskSources":
+    """The descriptors behind BASELINE configs[3]'s cache keys and task digests, for the 6124-TU trace looped to n
+    requests: per TU a source digest (64 hex chars, as the delegate's BLAKE3 of the preprocessed source) and one of
+    `n_args` invocation-argument strings whose lengths spread geometrically from about 100 B to 6 KiB, so that
+    messages end inside the first chunk and several chunks in.  Request i is TU i mod n_tus."""
+    from .dispatcher import TaskSources
+
+    rng = np.random.default_rng(seed)
+    words = ["-std=c++17", "-O2", "-g", "-fPIC", "-Wall", "-Wextra", "-DNDEBUG", "-fno-exceptions", "-pthread",
+             "-fvisibility=hidden", "-ffunction-sections", "-fdata-sections", "-march=x86-64-v2", "-c", "-x", "c++"]
+    args = []
+    for length in np.geomspace(100, 6144, n_args).astype(int):
+        parts: list[str] = []
+        while sum(len(x) + 1 for x in parts) < length:
+            parts.append(str(rng.choice(words)) if rng.random() < 0.6 else
+                         f"-I/src/llvm/{rng.bytes(6).hex()}/include" if rng.random() < 0.7 else f"-D{rng.bytes(4).hex().upper()}=1")
+        args.append(" ".join(parts)[:length])
+    tu_args = rng.integers(0, n_args, n_tus).astype(np.uint32)
+    tu_src = np.frombuffer(rng.bytes(32 * n_tus), dtype=np.uint8).reshape(n_tus, 32)
+    hexd = np.frombuffer(b"0123456789abcdef", dtype=np.uint8)
+    tu_hex = np.stack([hexd[tu_src >> 4], hexd[tu_src & 15]], axis=2).reshape(n_tus, 64)
+    tu = np.arange(n) % n_tus
+    return TaskSources.of(args, tu_args[tu], np.ascontiguousarray(tu_hex[tu]))
+
+
 def config_self(n_tasks: int = 100_000, n_servants: int = 2000, seed: int = 44, run_len: int = 4) -> Workload:
     """Production-like: ONE compiler digest, every requestor is itself a servant (so the
     self-exclusion rule, task_dispatcher.cc:372-379, is live for every request) and requests

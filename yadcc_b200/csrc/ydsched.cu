@@ -153,6 +153,8 @@ struct SolvePlan {
   uint32_t solver;        // 1 row scan, 2 slot streams
   uint32_t merge_rounds;  // (a graph key: a settled merge needs fewer)
   uint32_t force_stream;  // ClassTable::force_stream
+  // Flag 3 (the merge did not settle): eight times the rounds, at most as many as the merge has chunks (+ 2).
+  void MoreMergeRounds(uint32_t max_chunks) { merge_rounds = std::min(merge_rounds * 8, max_chunks + 2); }
 };
 
 // The solo kernel re-initialises the scratch it dirtied (class-table keys, zeroed region) before it ends; while this
@@ -966,6 +968,38 @@ uint32_t MergeChunk(const yd_sched* s, uint32_t Nb) {
   return !s->shard && Nb <= 262144 ? 256u : 512u;
 }
 
+// (class, slot) entries the slot lists hold per slot: a batch whose classes are eligible on more slots than that
+// overflows them (flag 1) and is decided by the row-scan solver.
+constexpr size_t kListEntriesPerSlot = 4;
+
+// The per-solve buffers of size class (Nb, slot_b) that both solvers and the sharded solve use.
+void EnsureSolveBuffers(yd_sched* s, uint32_t Nb, size_t slot_b) {
+  s->d_reqs.ensure(size_t(Nb) * sizeof(yd_task_req));
+  s->res_words = Nb;
+  s->d_res.ensure(size_t(Nb) * 4 + yd::kClsTableSize * 8);
+  s->d_out.ensure(size_t(Nb) * sizeof(yd_grant));
+  s->d_blk.ensure(size_t((Nb + 1023) / 1024) * 4);
+  s->d_row_off.ensure((s->sv.size() + 1) * 4);
+  s->d_row_len.ensure((s->sv.size() + 1) * 4);
+  s->d_codes.ensure(slot_b * (s->wide ? 8 : 4));
+  s->d_slot_owner.ensure(slot_b * 4);
+}
+
+// The call's scalars, in the host copy the solve uploads.
+const yd::DynParams& SetDynParams(yd_sched* s, uint32_t n, uint32_t slot_clamp, int64_t now_ns) {
+  return *s->h_dyn.as<yd::DynParams>() = yd::DynParams{n, slot_clamp, now_ns, s->lo, s->next_id};
+}
+
+// Flag 2 (more lists than provisioned): one list per class plus one pseudo-class list per merge-mode component are
+// needed, so the class bound doubles until it holds them, up to kMaxClasses.  False when it is there already.
+bool GrowClassBound(yd_sched* s, const uint32_t* meta) {
+  if (s->cls_bound >= yd::kMaxClasses) return false;
+  const uint32_t want = meta[0] + meta[2] + 1;
+  s->cls_bound *= 2;
+  while (s->cls_bound < want && s->cls_bound < yd::kMaxClasses) s->cls_bound *= 2;
+  return true;
+}
+
 // Allocates everything the slot-stream sequence touches for size class (Nb, slot_b) and
 // lays out the zero-initialised scratch region; called before a graph capture so that no
 // allocation happens inside it.
@@ -996,7 +1030,7 @@ void PrepareStreamBuffers(yd_sched* s, uint32_t Nb, size_t slot_b) {
   off += (size_t(s->cls_bound) * n_tiles + 1) * 4;
   s->z_bytes = (off + 255) & ~size_t(255);
   s->d_zero.ensure(s->z_bytes);
-  s->d_list.ensure(slot_b * 8 * 4);
+  s->d_list.ensure(slot_b * kListEntriesPerSlot * sizeof(uint2));
   s->d_list_bal.ensure(size_t(n_tiles) * s->cls_bound * 32 * 4);  // membership ballots: (tile, list, warp)
   // member lists of the fused solo solve: (tile, list, rank in the tile), for the batches the fused kernel may take --
   // cls_bound x tiles <= 32768, so 128 MiB at most (allocated here, before the scratch signature is taken: a buffer
@@ -1008,7 +1042,7 @@ void PrepareStreamBuffers(yd_sched* s, uint32_t Nb, size_t slot_b) {
   s->d_rcls.ensure(size_t(Nb) * 4); s->d_rrank.ensure(size_t(Nb) * 4); s->d_rq.ensure(size_t(Nb) * 8);
   s->d_rself.ensure(size_t(Nb) * 4);
   s->d_stream_scratch.ensure(std::max<size_t>(s->sv.size(), 1) * 8);
-  s->d_slot_pick.ensure(slot_b * 4 * 4);  // one word per list entry
+  s->d_slot_pick.ensure(slot_b * kListEntriesPerSlot * 4);  // one word per list entry
   // every slot is in at most one pseudo-class list: chunks <= slots / chunk + one partial chunk per list
   s->merge_max_chunks = (uint32_t)(slot_b / MergeChunk(s, Nb)) + s->cls_bound + 1;
   s->d_mst_in.ensure(size_t(s->merge_max_chunks) * yd::kMergeStateWords * 4);
@@ -1018,6 +1052,64 @@ void PrepareStreamBuffers(yd_sched* s, uint32_t Nb, size_t slot_b) {
     YD_CUDA_CHECK(cudaFuncSetAttribute(yd::k_solve_stream, cudaFuncAttributeMaxDynamicSharedMemorySize, 190 * 1024));
     s->stream_attr_set = true;
   }
+}
+
+// The tiling of one solve attempt of size class (Nb, slot_b), and its list counts in the zeroed scratch region (laid out
+// by PrepareStreamBuffers, so built after it).
+struct SolveGeometry {
+  uint32_t n_ltiles, n_rtiles;  // slot tiles (kListTile slots), request tiles (kRankTile requests)
+  size_t list_cap;              // entries of d_list
+  uint32_t* list_cnt;           // (class, slot tile) list counts
+};
+
+SolveGeometry MakeGeometry(yd_sched* s, uint32_t Nb, size_t slot_b) {
+  return SolveGeometry{(uint32_t)((slot_b + yd::kListTile - 1) / yd::kListTile), (Nb + yd::kRankTile - 1) / yd::kRankTile,
+                       slot_b * kListEntriesPerSlot,
+                       reinterpret_cast<uint32_t*>(static_cast<char*>(s->d_zero.p) + s->z_listcnt_off)};
+}
+
+// On `st`, after k_cls_insert: the final class table, each class's eligible servants, and the requests' FIFO ranks with
+// their scan.  `ev_fin` (if any) is recorded as soon as the class table is final.  Returns the kernels launched.
+uint32_t LaunchClassPhase(yd_sched* s, const SolveGeometry& g, const yd::TopoView& t, const yd::ClassTable& ct,
+                          cudaStream_t st, cudaEvent_t ev_fin) {
+  const yd::ServantArrays arr = s->arrays();
+  yd::k_cls_finalize<<<1, 1024, 0, st>>>(t, ct, arr, s->n_comps, s->d_comp_mode.as<uint32_t>());
+  if (ev_fin) YD_CUDA_CHECK(cudaEventRecord(ev_fin, st));
+  yd::k_cls_elig<<<ct.cls_bound, 256, 0, st>>>(t, ct, arr);
+  yd::k_rank_count<<<g.n_rtiles, yd::kRankTile, 0, st>>>(s->d_reqs.as<yd_task_req>(), s->d_dyn.as<yd::DynParams>(), t, ct,
+                                                          s->d_comp_mode.as<uint32_t>(), g.n_rtiles,
+                                                          s->d_rcls.as<uint32_t>(), s->d_rrank.as<uint32_t>(),
+                                                          s->d_rself.as<uint32_t>(), s->d_rank_cnt.as<uint32_t>());
+  yd::k_scan_rows<<<ct.cls_bound, 1024, 0, st>>>(s->d_rank_cnt.as<uint32_t>(), ct.meta, g.n_rtiles, ScanPub(s, 0));
+  return 4;
+}
+
+// On `st`, once the class table is final: the per-class slot lists, read through `dec`.  Returns the kernels launched.
+uint32_t LaunchListPhase(yd_sched* s, const SolveGeometry& g, const yd::SlotDecode& dec, const yd::TopoView& t,
+                         const yd::ClassTable& ct, cudaStream_t st) {
+  const unsigned long long* m_ptr = &s->d_counters.as<Counters>()->slots;
+  yd::k_list_count<<<g.n_ltiles, yd::kListTile, 0, st>>>(m_ptr, dec, t, ct, s->arrays(), g.n_ltiles, g.list_cnt,
+                                                         s->d_list_bal.as<uint32_t>());
+  yd::k_scan_rows<<<ct.cls_bound, 1024, 0, st>>>(g.list_cnt, ct.meta + 3, g.n_ltiles, ScanPub(s, 1));
+  yd::k_list_fill<<<g.n_ltiles, yd::kListTile, 0, st>>>(m_ptr, dec, t, ct, g.n_ltiles, g.list_cnt,
+                                                        s->d_list_bal.as<uint32_t>(), s->d_list.as<uint2>(),
+                                                        (uint32_t)g.list_cap);
+  return 3;
+}
+
+// The merge solver's arguments; LaunchMerge adds its launch shape.
+yd::MergeArgs MakeMergeArgs(yd_sched* s, const SolveGeometry& g, const yd::ClassTable& ct, const yd::RqLayout& L) {
+  yd::MergeArgs m{};
+  m.t = MakeTopo(s); m.ct = ct; m.mp = MakeMergePlan(s); m.sv = s->arrays(); m.dp = s->d_dyn.as<yd::DynParams>();
+  m.comp_mode = s->d_comp_mode.as<uint32_t>();
+  m.list_off = g.list_cnt; m.n_list_tiles = g.n_ltiles; m.list = s->d_list.as<uint2>();
+  m.rank_off = s->d_rank_cnt.as<uint32_t>(); m.n_rank_tiles = g.n_rtiles;
+  m.rq = s->d_rq.as<uint2>(); m.rcls = s->d_rcls.as<uint32_t>(); m.rself = s->d_rself.as<uint32_t>();
+  m.slot_pick = s->d_slot_pick.as<uint32_t>();
+  m.st_in = s->d_mst_in.as<uint32_t>(); m.st_out = s->d_mst_out.as<uint32_t>();
+  m.res = s->d_res.as<uint32_t>();
+  m.L = L;
+  return m;
 }
 
 // The merge solver: ONE persistent launch (rounds, scatter and check are phases behind grid barriers), so the
@@ -1072,55 +1164,34 @@ uint32_t RebuildSlotOrder(yd_sched* s, size_t slot_b) {
 
 // The solvers for everything the data-parallel path does not decide: the merge solver (all components but those with
 // several servants behind one requestor IP), then the sequential slot-stream walk for the rest.
-uint32_t LaunchCoupledSolvers(yd_sched* s, uint32_t N, size_t slot_b, const SolvePlan& plan, const yd::RqLayout& L) {
+uint32_t LaunchCoupledSolvers(yd_sched* s, uint32_t N, const SolveGeometry& g, const SolvePlan& plan, const yd::RqLayout& L) {
   cudaStream_t st = s->st;
-  uint32_t launches = 0;
-  yd::TopoView t = MakeTopo(s);
-  yd::ClassTable ct = MakeClassTable(s, plan);
-  yd::ServantArrays arr = s->arrays();
-  const yd::DynParams* dp = s->d_dyn.as<yd::DynParams>();
-  uint32_t* list_cnt = reinterpret_cast<uint32_t*>(static_cast<char*>(s->d_zero.p) + s->z_listcnt_off);
-  const uint32_t n_tiles = (uint32_t)((slot_b + yd::kListTile - 1) / yd::kListTile);
-  const uint32_t n_rtiles = (N + yd::kRankTile - 1) / yd::kRankTile;
   // ---- merge solver: everything but components with several servants behind one requestor IP -------
-  yd::MergePlan mp = MakeMergePlan(s);
-  {
-    yd::MergeArgs m{};
-    m.t = t; m.ct = ct; m.mp = mp; m.sv = arr; m.dp = dp;
-    m.comp_mode = s->d_comp_mode.as<uint32_t>();
-    m.list_off = list_cnt; m.n_list_tiles = n_tiles; m.list = s->d_list.as<uint2>();
-    m.rank_off = s->d_rank_cnt.as<uint32_t>(); m.n_rank_tiles = n_rtiles;
-    m.rq = s->d_rq.as<uint2>(); m.rcls = s->d_rcls.as<uint32_t>(); m.rself = s->d_rself.as<uint32_t>();
-    m.slot_pick = s->d_slot_pick.as<uint32_t>();
-    m.st_in = s->d_mst_in.as<uint32_t>(); m.st_out = s->d_mst_out.as<uint32_t>();
-    m.res = s->d_res.as<uint32_t>();
-    m.L = L;
-    launches += LaunchMerge(s, N, m, st);
-  }
+  yd::MergeArgs m = MakeMergeArgs(s, g, MakeClassTable(s, plan), L);
+  const uint32_t launches = LaunchMerge(s, N, m, st);
 
   // ---- sequential decisions for everything else ---------------------------------------------
   yd::StreamArgs a{};
   a.reqs = s->d_reqs.as<yd_task_req>();
-  a.dp = dp;
+  a.dp = m.dp;
   a.res = s->d_res.as<uint32_t>();
-  a.t = t;
-  a.ct = ct;
-  a.sv = arr;
+  a.t = m.t;
+  a.ct = m.ct;
+  a.sv = m.sv;
   a.row_len = s->d_row_len.as<uint32_t>();
   a.static_rows = s->order_static ? 1u : 0u;
-  a.list_off = list_cnt;
-  a.n_list_tiles = n_tiles;
+  a.list_off = g.list_cnt;
+  a.n_list_tiles = g.n_ltiles;
   a.list = s->d_list.as<uint2>();
   a.max_comp_servants = (uint32_t)std::min<size_t>(s->max_comp_servants, kStreamMaxComponent);
   a.gscratch = s->d_stream_scratch.as<uint32_t>();
   a.n_servants = (uint32_t)s->sv.size();
   a.comp_mode = s->d_comp_mode.as<uint32_t>();
-  a.viol = mp.viol;
+  a.viol = m.mp.viol;
   a.counters = s->d_counters.as<Counters>();
   const size_t dyn = size_t(a.max_comp_servants) * 8;
   yd::k_solve_stream<<<s->n_comps, (yd::kStreamProducers + 1) * 32, dyn, st>>>(a);
-  launches += 1;
-  return launches;
+  return launches + 1;
 }
 
 // `st` waits for the request upload on the copy stream: when this call copied requests (`copied`), and always in a
@@ -1134,16 +1205,13 @@ void WaitUpload(yd_sched* s, cudaStream_t st, bool copied, bool capturing) {
 //   st  : slot table (+ first histogram) -> radix passes
 //   st2 : [wait for the request upload] class table -> finalize -> FIFO ranks -> scan
 // joined before the per-class lists.
-uint32_t LaunchStream(yd_sched* s, uint32_t N, size_t slot_b, const SolvePlan& plan, bool copied, bool capturing) {
+uint32_t LaunchStream(yd_sched* s, uint32_t N, const SolveGeometry& g, const SolvePlan& plan, bool copied, bool capturing) {
   cudaStream_t st = s->st, st2 = s->st2;
   uint32_t launches = 0;
   yd::TopoView t = MakeTopo(s);
   yd::ClassTable ct = MakeClassTable(s, plan);
   yd::ServantArrays arr = s->arrays();
   const yd::DynParams* dp = s->d_dyn.as<yd::DynParams>();
-  uint32_t* list_cnt = reinterpret_cast<uint32_t*>(static_cast<char*>(s->d_zero.p) + s->z_listcnt_off);
-  const uint32_t n_tiles = (uint32_t)((slot_b + yd::kListTile - 1) / yd::kListTile);
-  const uint32_t n_rtiles = (N + yd::kRankTile - 1) / yd::kRankTile;
 
   // ---- fork ---------------------------------------------------------------------
   YD_CUDA_CHECK(cudaEventRecord(s->ev_fork, st));
@@ -1151,16 +1219,8 @@ uint32_t LaunchStream(yd_sched* s, uint32_t N, size_t slot_b, const SolvePlan& p
   // branch B: classes and FIFO ranks (needs the requests in HBM)
   WaitUpload(s, st2, copied, capturing);
   yd::k_cls_insert<<<(N + 255) / 256, 256, 0, st2>>>(s->d_reqs.as<yd_task_req>(), dp, t, ct);
-  yd::k_cls_finalize<<<1, 1024, 0, st2>>>(t, ct, arr, s->n_comps, s->d_comp_mode.as<uint32_t>());
-  YD_CUDA_CHECK(cudaEventRecord(s->ev_fin, st2));  // the list kernels on `st` need the class table, not what follows
-  yd::k_cls_elig<<<ct.cls_bound, 256, 0, st2>>>(t, ct, arr);
-  yd::k_rank_count<<<n_rtiles, yd::kRankTile, 0, st2>>>(s->d_reqs.as<yd_task_req>(), dp, t, ct,
-                                                         s->d_comp_mode.as<uint32_t>(), n_rtiles,
-                                                         s->d_rcls.as<uint32_t>(), s->d_rrank.as<uint32_t>(),
-                                                         s->d_rself.as<uint32_t>(), s->d_rank_cnt.as<uint32_t>());
-  yd::k_scan_rows<<<ct.cls_bound, 1024, 0, st2>>>(s->d_rank_cnt.as<uint32_t>(), ct.meta, n_rtiles, ScanPub(s, 0));
+  launches += 1 + LaunchClassPhase(s, g, t, ct, st2, s->ev_fin);  // (the list kernels on `st` wait for ev_fin alone)
   YD_CUDA_CHECK(cudaEventRecord(s->ev_join, st2));
-  launches += 5;
   // branch A: slot table and its sort -- unless the kept (static) order is valid
   if (!s->order_static) {
     launches += LaunchSlotTable(s, true);
@@ -1170,48 +1230,40 @@ uint32_t LaunchStream(yd_sched* s, uint32_t N, size_t slot_b, const SolvePlan& p
   YD_CUDA_CHECK(cudaStreamWaitEvent(st, s->ev_fin, 0));
 
   // ---- per-class sorted slot lists ----------------------------------------------------
-  const unsigned long long* m_ptr = &s->d_counters.as<Counters>()->slots;
-  yd::SlotDecode dec{s->d_sort_v[0].as<uint32_t>(), s->d_slot_owner.as<uint32_t>(), s->d_row_off.as<uint32_t>(),
-                     s->d_row_len.as<uint32_t>(), s->d_run.as<uint32_t>(), s->order_static ? 1u : 0u,
-                     s->order_static ? s->d_slot_rec.as<uint2>() : nullptr};
-  yd::k_list_count<<<n_tiles, yd::kListTile, 0, st>>>(m_ptr, dec, t, ct, arr, n_tiles, list_cnt,
-                                                      s->d_list_bal.as<uint32_t>());
-  yd::k_scan_rows<<<ct.cls_bound, 1024, 0, st>>>(list_cnt, ct.meta + 3, n_tiles, ScanPub(s, 1));
-  yd::k_list_fill<<<n_tiles, yd::kListTile, 0, st>>>(m_ptr, dec, t, ct, n_tiles, list_cnt, s->d_list_bal.as<uint32_t>(),
-                                                     s->d_list.as<uint2>(), (uint32_t)(slot_b * 4));
-  launches += 3;
+  const yd::SlotDecode dec{s->d_sort_v[0].as<uint32_t>(), s->d_slot_owner.as<uint32_t>(), s->d_row_off.as<uint32_t>(),
+                           s->d_row_len.as<uint32_t>(), s->d_run.as<uint32_t>(), s->order_static ? 1u : 0u,
+                           s->order_static ? s->d_slot_rec.as<uint2>() : nullptr};
+  launches += LaunchListPhase(s, g, dec, t, ct, st);
 
   // ---- join: FIFO ranks and eligibility counts are needed from here on ---------------------------------------
   YD_CUDA_CHECK(cudaStreamWaitEvent(st, s->ev_join, 0));
   // ---- data-parallel path: single-class components without self-requests ----------------
   // (n_local = the grid bound: res[] has that many cells and only requests < dp->n are ever named)
   const yd::RqLayout L = MakeRqLayout(s, 0, N, false);
-  yd::k_rank_assign<<<(N + 255) / 256, 256, 0, st>>>(dp, n_rtiles, t, ct, s->d_rcls.as<uint32_t>(),
+  yd::k_rank_assign<<<(N + 255) / 256, 256, 0, st>>>(dp, g.n_rtiles, t, ct, s->d_rcls.as<uint32_t>(),
                                                      s->d_rrank.as<uint32_t>(), s->d_rself.as<uint32_t>(),
-                                                     s->d_rank_cnt.as<uint32_t>(), list_cnt,
-                                                     n_tiles, s->d_list.as<uint2>(), arr, s->d_comp_mode.as<uint32_t>(),
+                                                     s->d_rank_cnt.as<uint32_t>(), g.list_cnt,
+                                                     g.n_ltiles, s->d_list.as<uint2>(), arr, s->d_comp_mode.as<uint32_t>(),
                                                      s->d_rq.as<uint2>(), s->d_res.as<uint32_t>(), L);
   launches += 1;
 
-  launches += LaunchCoupledSolvers(s, N, slot_b, plan, L);
+  launches += LaunchCoupledSolvers(s, N, g, plan, L);
   return launches;
 }
 
 // The solo kernel searches the scanned list offsets, cls_bound x (slot tiles + 1) + 1 words, once per request.  When they
 // fit in dynamic shared memory (64 KB at most) every block derives the offsets it needs from the raw counts, without
 // the leader scans of E2 (fused.cuh); the speculative variant needs that.  Returns the words, 0 when they do not fit.
-uint32_t FusedLoffWords(const yd_sched* s, size_t slot_b) {
-  const size_t cells = size_t(s->cls_bound) * ((slot_b + yd::kListTile - 1) / yd::kListTile + 1) + 1;
+uint32_t FusedLoffWords(const yd_sched* s, const SolveGeometry& g) {
+  const size_t cells = size_t(s->cls_bound) * (g.n_ltiles + 1) + 1;
   return cells <= 16384 ? (uint32_t)cells : 0u;
 }
 
 // The arguments of the fused front kernel (fused.cuh) for a batch of size class N.  `capturing` (general variants only):
 // the scalars come through a copy node enqueued here; a solo launch, never graphed, gets them as kernel parameters.
-yd::FusedArgs MakeFusedArgs(yd_sched* s, uint32_t N, size_t slot_b, const SolvePlan& plan, bool capturing, bool packed_in,
-                            bool packed_out) {
+yd::FusedArgs MakeFusedArgs(yd_sched* s, uint32_t N, const SolveGeometry& g, const SolvePlan& plan, bool capturing,
+                            bool packed_in, bool packed_out) {
   const bool solo = IsSolo(plan.variant);
-  const uint32_t n_tiles = (uint32_t)((slot_b + yd::kListTile - 1) / yd::kListTile);
-  const uint32_t n_rtiles = (N + yd::kRankTile - 1) / yd::kRankTile;
   yd::FusedArgs a{};
   a.sc = s->fsc;
   a.sc_dev = (capturing && !solo) ? s->d_fsc.as<yd::FusedScalars>() : nullptr;
@@ -1233,17 +1285,17 @@ yd::FusedArgs MakeFusedArgs(yd_sched* s, uint32_t N, size_t slot_b, const SolveP
   a.m_ptr = &s->d_counters.as<Counters>()->slots;
   a.comp_mode = s->d_comp_mode.as<uint32_t>();
   a.n_comps = s->n_comps;
-  a.n_rtiles = n_rtiles;
-  a.n_ltiles = n_tiles;
+  a.n_rtiles = g.n_rtiles;
+  a.n_ltiles = g.n_ltiles;
   a.rcls = s->d_rcls.as<uint32_t>();
   a.rrank = s->d_rrank.as<uint32_t>();
   a.rself = s->d_rself.as<uint32_t>();
   a.rank_cnt = s->d_rank_cnt.as<uint32_t>();
-  a.list_cnt = reinterpret_cast<uint32_t*>(static_cast<char*>(s->d_zero.p) + s->z_listcnt_off);
+  a.list_cnt = g.list_cnt;
   a.list_bal = s->d_list_bal.as<uint32_t>();
   a.members = s->d_members.as<uint32_t>();
   a.list = s->d_list.as<uint2>();
-  a.list_cap = (uint32_t)(slot_b * 4);
+  a.list_cap = (uint32_t)g.list_cap;
   a.rq = s->d_rq.as<uint2>();
   a.res = s->d_res.as<uint32_t>();
   a.L = MakeRqLayout(s, 0, N, false);
@@ -1256,7 +1308,7 @@ yd::FusedArgs MakeFusedArgs(yd_sched* s, uint32_t N, size_t slot_b, const SolveP
   a.counters = s->d_counters.as<Counters>();
   a.n_servants = (uint32_t)s->sv.size();
   a.prof = s->fused_prof ? s->d_fused_prof.as<unsigned long long>() : nullptr;
-  a.loff_cache_words = solo ? FusedLoffWords(s, slot_b) : 0u;
+  a.loff_cache_words = solo ? FusedLoffWords(s, g) : 0u;
   a.spec = plan.variant == kSoloSpec ? 1u : 0u;
   a.kept_env = s->d_kept_env.as<uint4>();
   a.kept_sv = s->d_kept_sv.as<uint32_t>();
@@ -1272,12 +1324,12 @@ void LaunchFusedKernel(yd_sched* s, const yd::FusedArgs& a) {
 }
 
 // A general (not solo) fused solve: the fused front kernel, then the coupled solvers.
-uint32_t LaunchFused(yd_sched* s, uint32_t N, size_t slot_b, const SolvePlan& plan, bool copied, bool capturing, bool packed_in,
-                     bool packed_out) {
-  const yd::FusedArgs a = MakeFusedArgs(s, N, slot_b, plan, capturing, packed_in, packed_out);
+uint32_t LaunchFused(yd_sched* s, uint32_t N, const SolveGeometry& g, const SolvePlan& plan, bool copied, bool capturing,
+                     bool packed_in, bool packed_out) {
+  const yd::FusedArgs a = MakeFusedArgs(s, N, g, plan, capturing, packed_in, packed_out);
   WaitUpload(s, s->st, copied, capturing);
   LaunchFusedKernel(s, a);
-  return 1 + LaunchCoupledSolvers(s, N, slot_b, plan, a.L);
+  return 1 + LaunchCoupledSolvers(s, N, g, plan, a.L);
 }
 
 }  // namespace
@@ -1296,8 +1348,8 @@ uint64_t NextPow2(uint64_t v, uint64_t lo) {
 // solve: the sequence that is captured into a CUDA graph.  (A solo solve is one kernel: WaitImpl launches it.)
 // packed bit 0: the upload is 16-byte records in d_reqs16; bit 1: the download is 8-byte grants from d_out8.
 // `copied`: this call copied the requests on the copy stream (WaitUpload).
-uint32_t EnqueueSolve(yd_sched* s, uint32_t Nb, size_t slot_b, const SolvePlan& plan, bool record_events, bool copied,
-                      bool capturing, uint32_t packed) {
+uint32_t EnqueueSolve(yd_sched* s, uint32_t Nb, const SolveGeometry& g, const SolvePlan& plan, bool record_events,
+                      bool copied, bool capturing, uint32_t packed) {
   cudaStream_t st = s->st;
   const uint32_t S = (uint32_t)s->sv.size();
   const uint32_t solver = plan.solver;
@@ -1322,8 +1374,8 @@ uint32_t EnqueueSolve(yd_sched* s, uint32_t Nb, size_t slot_b, const SolvePlan& 
   }
   if (have_work && solver == 2) {
     if (record_events) YD_CUDA_CHECK(cudaEventRecord(s->ev[2], st));
-    if (fused) launches += LaunchFused(s, Nb, slot_b, plan, copied, capturing, packed_in, packed_out);
-    else launches += LaunchStream(s, Nb, slot_b, plan, copied, capturing);
+    if (fused) launches += LaunchFused(s, Nb, g, plan, copied, capturing, packed_in, packed_out);
+    else launches += LaunchStream(s, Nb, g, plan, copied, capturing);
     abort_flag = MakeClassTable(s, plan).meta + 1;
   } else {
     if (have_work) launches += LaunchSlotTable(s, false);
@@ -1472,17 +1524,9 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
   const size_t slot_b = (size_t)NextPow2(std::max<size_t>(slot_bound, 1), 4096);
   if (!want_static) s->order_static = false;
   const uint32_t nb = (Nb + 1023) / 1024;
-  s->d_reqs.ensure(size_t(Nb) * sizeof(yd_task_req));
-  s->res_words = Nb;
-  s->d_res.ensure(size_t(Nb) * 4 + yd::kClsTableSize * 8);
-  s->d_out.ensure(size_t(Nb) * sizeof(yd_grant));
+  EnsureSolveBuffers(s, Nb, slot_b);
   if (reqs16) s->d_reqs16.ensure(size_t(Nb) * sizeof(yd_task_req16));
   if (out8) s->d_out8.ensure(size_t(Nb) * sizeof(yd_grant8));
-  s->d_blk.ensure(size_t(nb) * 4);
-  s->d_row_off.ensure(size_t(S + 1) * 4);
-  s->d_row_len.ensure(size_t(S + 1) * 4);
-  s->d_codes.ensure(slot_b * (s->wide ? 8 : 4));
-  s->d_slot_owner.ensure(slot_b * 4);
 
   // solver choice: 2 (slot streams) unless asked otherwise or a component is too big for it
   // (the slot-stream solver takes components of any size: its sequential fallback keeps running_tasks of a
@@ -1491,13 +1535,7 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
   SolvePlan plan{kPipeline, s->solver_pref == 1 && s->max_comp_servants <= kRowscanMaxComponent ? 1u : 2u,
                  s->cfg_merge_rounds, s->cfg_force_stream};
 
-  yd::DynParams* hd = s->h_dyn.as<yd::DynParams>();
-  hd->n = N;
-  hd->slot_clamp = N;
-  hd->now_ns = now_ns;
-  hd->ring_lo = s->lo;
-  hd->ring_next = s->next_id;
-  s->fsc.dyn = *hd;
+  s->fsc.dyn = SetDynParams(s, N, N, now_ns);
 
   uint32_t launches = 0;
   hp[1] = hp_now();
@@ -1536,24 +1574,25 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
   for (;;) {
     memset(s->h_meta.p, 0, 32);
     graphed = false;
+    // every buffer the sequence touches exists BEFORE a capture (no allocation inside one), and the scratch layout the
+    // kept signature below describes is fixed
+    if (plan.solver == 2) PrepareStreamBuffers(s, Nb, slot_b);
+    const SolveGeometry geo = MakeGeometry(s, Nb, slot_b);
     // The fused front kernel takes batches in the latency-bound regime whose (class, tile) count matrices one block
     // scans in a few rounds; it needs the kept slot order.  Solo = it also writes the grants (no coupled component
     // had requests last time; if one has now, the kernel raises flag 4 and the batch is replayed with kFused).
     const bool fused = s->fused_cfg && s->fused_grid && s->solver_pref == 0 && plan.solver == 2 && want_static && S &&
-                       s->n_comps && Nb <= s->fused_max_nb &&
-                       size_t(s->cls_bound) * ((Nb + yd::kRankTile - 1) / yd::kRankTile) <= 32768 &&
-                       size_t(s->cls_bound) * ((slot_b + yd::kListTile - 1) / yd::kListTile) <= 32768;
+                       s->n_comps && Nb <= s->fused_max_nb && size_t(s->cls_bound) * geo.n_rtiles <= 32768 &&
+                       size_t(s->cls_bound) * geo.n_ltiles <= 32768;
     KeptSig now;
     if (fused && s->solo.hint) {
-      PrepareStreamBuffers(s, Nb, slot_b);  // (fixes the scratch layout the signature describes)
       now = KeptSig{CleanSig{g_buf_generation, s->z_cls_off, s->z_bytes, s->res_words, s->d_zero.p, s->d_res.p},
                     s->topo_gen, s->cls_bound};
     }
     // speculative (fused.cuh): every block holds at most two request tiles (their classes and ranks stay in
     // registers), the lists' offsets fit in shared memory, and registry positions fit the member words below the slot's
     // index in its tile (classes.cuh: kMemberSlotShift)
-    const bool spec_ok = FusedLoffWords(s, slot_b) != 0 && (Nb + yd::kRankTile - 1) / yd::kRankTile <= 2 * s->fused_grid &&
-                         S <= yd::kMemberPosMask;
+    const bool spec_ok = FusedLoffWords(s, geo) != 0 && geo.n_rtiles <= 2 * s->fused_grid && S <= yd::kMemberPosMask;
     plan.variant = s->solo.Choose(fused, now, spec_ok);
     // (a staged solve -- no request array in this call -- leaves its grants in HBM and copies them afterwards, so that
     // the device-side events around it time the solve alone)
@@ -1567,8 +1606,6 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
     s->fsc.kept_fp = s->solo.kept_fp;
     *s->h_fsc.as<yd::FusedScalars>() = s->fsc;
     s->h_fio->done_seq = 0;
-    // every buffer the sequence touches exists BEFORE a capture (no allocation inside one)
-    if (plan.solver == 2) PrepareStreamBuffers(s, Nb, slot_b);
     if (plan.solver == 2 && want_static && S && s->n_comps && (s->order_dirty || !s->order_static || s->order_slot_b != slot_b)) {
       launches += RebuildSlotOrder(s, slot_b);
     }
@@ -1576,7 +1613,7 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
       // ONE kernel whose per-call scalars are kernel parameters: launched directly, as a graph would add a parameter
       // patch and a graph launch to the call.  Its arguments are built before the events, which bracket what the solve
       // enqueues on `st`; the kernel leaves grant count and flags in the mapped host record.
-      const yd::FusedArgs a = MakeFusedArgs(s, Nb, slot_b, plan, false, packed & 1u, packed & 2u);
+      const yd::FusedArgs a = MakeFusedArgs(s, Nb, geo, plan, false, packed & 1u, packed & 2u);
       hp[3] = hp_now();
       YD_CUDA_CHECK(cudaEventRecord(s->ev[1], st));
       if (plan.variant == kSolo) {
@@ -1604,7 +1641,7 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
       if (!hit) {
         cudaGraph_t graph = nullptr;
         YD_CUDA_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-        uint32_t l = EnqueueSolve(s, Nb, slot_b, plan, false, copied, true, packed);
+        uint32_t l = EnqueueSolve(s, Nb, geo, plan, false, copied, true, packed);
         YD_CUDA_CHECK(cudaStreamEndCapture(st, &graph));
         cudaGraphExec_t exec = nullptr;
         YD_CUDA_CHECK(cudaGraphInstantiate(&exec, graph, 0));
@@ -1624,7 +1661,7 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
       launches += hit->launches;
       graphed = true;
     } else {
-      launches += EnqueueSolve(s, Nb, slot_b, plan, true, copied, false, packed);
+      launches += EnqueueSolve(s, Nb, geo, plan, true, copied, false, packed);
     }
     if (plan.solver == 1) { s->order_dirty = true; s->order_static = false; }  // the row-scan solver's table overwrote the kept one
     if (zc_out) {}  // the kernel wrote the grants into the caller's page-locked array
@@ -1667,21 +1704,18 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
     s->solo.Take(plan.variant, meta, now, s->h_fio->classes_fp);
     if (plan.solver == 2 && S && s->n_comps && meta[1] != 0) {
       // Nothing was decided (the stream solver and the final kernels all stood down).
-      const uint32_t flag = meta[1], ncls = meta[0];
+      const uint32_t flag = meta[1];
       if (flag == yd::kFlagSpecMiss) {
         // the kept class table could not decide the batch: replay without speculation (which builds the table again)
         spec = 2;
       } else if (flag == 4) {
         // the solo kernel met a component it cannot decide: the general sequence, now and next time (SoloTables::Take)
-      } else if (flag == 2 && grow_attempts++ < 3 && s->cls_bound < yd::kMaxClasses) {  // more lists than provisioned: grow and go again
-        // one list per class plus one pseudo-class list per merge-mode component
-        const uint32_t want = ncls + meta[2] + 1;
-        s->cls_bound *= 2;
-        while (s->cls_bound < want && s->cls_bound < yd::kMaxClasses) s->cls_bound *= 2;
+      } else if (flag == 2 && grow_attempts++ < 3 && GrowClassBound(s, meta)) {
+        // more lists than provisioned: go again with the grown class bound
       } else if (flag == 3 && merge_retry < 2) {
         // the merge solver's boundary states had not settled after the rounds in the graph: more
         // rounds first, then the sequential solver for everything it would have decided
-        if (merge_retry == 0) plan.merge_rounds = std::min(plan.merge_rounds * 8, s->merge_max_chunks + 2);
+        if (merge_retry == 0) plan.MoreMergeRounds(s->merge_max_chunks);
         else plan.force_stream = 2;
         ++merge_retry;
       } else {

@@ -4,13 +4,15 @@
 #   make cuda       -> yadcc_b200/libydsched.so
 #   make oracle     -> the checkers (+ checkers/libydport_state.so: the port with the state export / import,
 #                      checkers/libydport_keys.so and oracle/_ref/libydref_keys.so: port and reference with the task keys)
+#   make fake_nccl  -> tests/fake_nccl/libnccl.so.2: the test-only NCCL stand-in that runs several ranks of the
+#                      range-sharded scheduler as threads of one process on one GPU (tests/test_shard_one_gpu.py)
 NVCC ?= /usr/local/cuda/bin/nvcc
 ARCH = -gencode arch=compute_90a,code=sm_90a
 NVCCFLAGS = -O3 -std=c++17 -lineinfo $(ARCH) -Xcompiler -fPIC,-Wall,-Wno-unused-function -Iinclude -Iyadcc_b200/csrc
 CSRC = yadcc_b200/csrc
 LIB = yadcc_b200/libydsched.so
 
-all: cuda oracle
+all: cuda oracle fake_nccl
 
 cuda: $(LIB)
 
@@ -27,8 +29,14 @@ checkers/libydport_state.so: checkers/port_state.cc oracle/port.cc include/ydsta
 checkers/libydport_keys.so: checkers/port_keys.cc oracle/port.cc include/ydsched.h include/ydkeys.h $(wildcard include/*.inc)
 	$(CXX) -std=gnu++2a -O2 -fPIC -Wall -Wno-sign-compare -Wno-unused-variable -Wno-subobject-linkage -Iinclude -shared -o $@ checkers/port_keys.cc
 
+FAKE_NCCL = tests/fake_nccl/libnccl.so.2
+fake_nccl: $(FAKE_NCCL)
+
+$(FAKE_NCCL): tests/fake_nccl/fake_nccl.cc
+	$(CXX) -std=c++17 -O2 -fPIC -Wall -shared -Wl,-soname,libnccl.so.2 -o $@ $< -ldl -pthread
+
 clean:
-	rm -f $(LIB) checkers/libydport_state.so checkers/libydport_keys.so oracle/_ref/libydref_keys.so
+	rm -f $(LIB) $(FAKE_NCCL) checkers/libydport_state.so checkers/libydport_keys.so oracle/_ref/libydref_keys.so
 	$(MAKE) -C oracle clean
 
-.PHONY: all cuda oracle clean
+.PHONY: all cuda oracle fake_nccl clean

@@ -17,7 +17,10 @@
  * Between 3 and 4 every rank runs the same slot-side merge (solve_merge.cuh) on the same data and
  * keeps the verdicts of its own requests.  Task ids are the batch's FIFO ordinals (rank g's grants
  * follow those of the lower ranks).  Leases (TaskDesc, task_dispatcher.h:199-215) live on the rank
- * that holds the request; FreeTask is collective so that running_tasks stays replicated.
+ * that holds the request, so a zombie swept by a heartbeat or a freed lease lowers running_tasks on
+ * that rank first; each rank counts those decrements and the next collective call (exchange 1 of a
+ * solve, or yd_shard_free_tasks) hands them to the others.  After every collective call every rank's
+ * running_tasks is the single scheduler's; in between, a non-holder rank's may be higher.
  *
  * The library dlopen()s libnccl.so.2 on yd_shard_init: a single-GPU process never needs it.
  */
@@ -43,15 +46,18 @@ void yd_shard_finalize(yd_sched* s);
 /* Collective, THE HOT PATH: the whole queue = ranks' `reqs_local` concatenated in rank order.  out_local[i]
  * is what the i-th request of this rank's range gets (same fields as yd_wait_for_starting_new_tasks;
  * task ids number the grants of the whole batch in FIFO order).  reqs_local == NULL: the range staged with
- * yd_stage_requests.  Returns 0; 2 if some digest component needs the sequential solver (several servants
- * behind one requestor IP, more than 32 classes on one component, or the last-resort rule fired) -- nothing
- * was decided then and every rank gets the same answer, the caller solves that batch on one rank. */
+ * yd_stage_requests.  A batch with a component that needs the sequential solver (several servants behind one
+ * requestor IP, more than 32 classes on one component, the last-resort rule, a request beyond the exchange-3
+ * margin) is decided by every rank: the ranges are gathered and every rank runs the ordinary solve on the
+ * whole queue, keeping its own range's grants and leases.  Returns 0; 1 (on every rank, nothing exchanged or
+ * changed) if the cluster has capacities above 8192 per servant, or if reqs_local == NULL and n_local is
+ * larger than the staged queue. */
 int yd_shard_wait_for_starting_new_tasks(yd_sched* s, int64_t now_ns, const yd_task_req* reqs_local, size_t n_local,
                                          yd_grant* out_local);
 
 /* Collective FreeTask x n (task_dispatcher.cc:167-188): every rank passes the ids IT wants freed (any
- * subset, also none); a lease is released by the rank that holds it and the running_tasks decrements
- * reach every replica through one all-reduce. */
+ * subset, also none, also ids another rank holds); the ids are gathered, a lease is released by the rank
+ * that holds it and the running_tasks decrements reach every replica through one all-reduce. */
 int yd_shard_free_tasks(yd_sched* s, const uint64_t* ids, size_t n);
 
 /* Device time (ms, CUDA events on the solve stream) of the last sharded solve's phases: local kernels and

@@ -63,17 +63,18 @@ __global__ void __launch_bounds__(1024) k_shard_count_grants(const uint32_t* __r
   if (threadIdx.x == 0) *cell = s_sum;
 }
 
-// running_tasks deltas of a collective FreeTask: delta = snapshot - run (what this rank released) ...
-__global__ void k_run_delta(uint32_t S, const uint32_t* __restrict__ snap, const uint32_t* __restrict__ run,
-                            uint32_t* __restrict__ delta) {
+// running_tasks decrements made on one rank only -- a lease lives on the rank that holds its request, so a zombie
+// swept by a heartbeat (k_notify_sweep) or a freed lease (k_free) lowers running_tasks there first -- reach the other
+// ranks at the next collective call: `parts` holds every rank's decrements (`nparts` arrays `stride` words apart, or
+// their sum), `dec` this rank's own, already applied to `run`.
+__global__ void k_run_reconcile(uint32_t S, const uint32_t* __restrict__ parts, size_t stride, uint32_t nparts,
+                                uint32_t* __restrict__ dec, uint32_t* __restrict__ run) {
   const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
-  if (s < S) delta[s] = snap[s] - run[s];
-}
-// ... and run = snapshot - (sum of everybody's releases).
-__global__ void k_run_apply(uint32_t S, const uint32_t* __restrict__ snap, const uint32_t* __restrict__ delta_sum,
-                            uint32_t* __restrict__ run) {
-  const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
-  if (s < S) run[s] = snap[s] - delta_sum[s];
+  if (s >= S) return;
+  uint32_t all = 0;
+  for (uint32_t g = 0; g < nparts; ++g) all += parts[g * stride + s];
+  run[s] -= all - dec[s];
+  dec[s] = 0;
 }
 
 }  // namespace yd

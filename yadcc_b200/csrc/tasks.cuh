@@ -278,8 +278,11 @@ __global__ void k_apply_claims(uint32_t S, const uint32_t* __restrict__ claims, 
 }
 
 // ---- FreeTask (cc:167-188), one thread per id --------------------------------
+// `dec` (range-sharded handles only, else null): this rank's running_tasks decrements since the last collective
+// call, which hands them to the other ranks (shard_host.inc).  run == null: the lease is forgotten, running_tasks
+// stays (a lease another rank holds, shard_host.inc).
 __global__ void k_free(const unsigned long long* __restrict__ ids, uint32_t n, TaskRing ring,
-                       uint32_t* __restrict__ run, Counters* __restrict__ counters) {
+                       uint32_t* __restrict__ run, Counters* __restrict__ counters, uint32_t* __restrict__ dec) {
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   unsigned long long id;
@@ -287,7 +290,8 @@ __global__ void k_free(const unsigned long long* __restrict__ ids, uint32_t n, T
   uint64_t slot = id & ring.mask;
   uint32_t old = atomicExch(&ring.flags[slot], 0u);  // duplicates in one call: first one wins
   if (old & kTaskAlive) {
-    atomicSub(&run[ring.srv[slot]], 1u);
+    if (run) atomicSub(&run[ring.srv[slot]], 1u);
+    if (dec) atomicAdd(&dec[ring.srv[slot]], 1u);
     atomicAdd(&counters->alive, ~0ull);
     if (old & kTaskZombie) atomicAdd(&counters->zombies, ~0ull);
   }
@@ -384,13 +388,15 @@ __global__ void k_compact_servants(uint32_t S_old, const uint32_t* __restrict__ 
                                    const uint32_t* __restrict__ run_old,
                                    const unsigned long long* __restrict__ ever_old,
                                    uint32_t* __restrict__ run_new,
-                                   unsigned long long* __restrict__ ever_new) {
+                                   unsigned long long* __restrict__ ever_new,
+                                   const uint32_t* __restrict__ dec_old, uint32_t* __restrict__ dec_new) {
   uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
   if (s >= S_old) return;
   uint32_t np = remap[s];
   if (np != kNone) {
     run_new[np] = run_old[s];
     ever_new[np] = ever_old[s];
+    if (dec_new) dec_new[np] = dec_old[s];
   }
 }
 
@@ -417,9 +423,9 @@ __device__ __forceinline__ uint32_t notify_find_item(const NotifyBatch& b, uint3
 
 // Sweep: zombies of a heartbeating servant that the servant no longer reports are freed
 // (UnsafeSweepZombiesOf, cc:453-476).  One thread per lease of the live window; zombies are rare,
-// so the scan of the servant's reported ids (global memory, any length) is off the common path.
+// so the scan of the servant's reported ids (global memory, any length) is off the common path.  `dec` as in k_free.
 __global__ void k_notify_sweep(TaskRing ring, NotifyBatch b, uint32_t* __restrict__ run,
-                               Counters* __restrict__ counters) {
+                               Counters* __restrict__ counters, uint32_t* __restrict__ dec) {
   unsigned long long id = ring.lo + (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (id >= ring.next) return;
   uint64_t slot = id & ring.mask;
@@ -434,6 +440,7 @@ __global__ void k_notify_sweep(TaskRing ring, NotifyBatch b, uint32_t* __restric
   }
   ring.flags[slot] = 0;
   atomicSub(&run[pos], 1u);
+  if (dec) atomicAdd(&dec[pos], 1u);
   atomicAdd(&counters->alive, ~0ull);
   atomicAdd(&counters->zombies, ~0ull);
 }

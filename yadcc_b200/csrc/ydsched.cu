@@ -13,6 +13,7 @@
 //
 // There is no CPU fallback: yd_create fails without an sm_90 device.
 #include <algorithm>
+#include <atomic>
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
@@ -49,8 +50,9 @@ using yd::kNone;
 
 // ---- small helpers ---------------------------------------------------------
 
-// Bumped whenever any device buffer moves: captured graphs hold raw pointers.
-static unsigned long long g_buf_generation = 0;
+// Bumped whenever any device buffer moves: captured graphs hold raw pointers.  (Atomic: several handles may run
+// in threads of one process, e.g. the ranks of a range-sharded scheduler.)
+static std::atomic<unsigned long long> g_buf_generation{0};
 
 struct DevBuf {  // grow-only device allocation
   void* p = nullptr;
@@ -248,6 +250,7 @@ struct yd_sched {
   // device servant arrays; state (run/ever) is valid for positions < S_dev
   DevBuf d_nproc, d_load, d_maxt, d_flags, d_ver, d_run, d_ever;
   DevBuf d_run_tmp, d_ever_tmp, d_remap;
+  DevBuf d_dec, d_dec_tmp;  // range-sharded handles: running_tasks decrements not yet handed to the other ranks
   uint32_t S_dev = 0;
   PinBuf h_facts;
 
@@ -422,6 +425,10 @@ void yd_sched::SyncServantState() {
   d_ever.ensure(size_t(S) * 8, true, st);
   YD_CUDA_CHECK(cudaMemsetAsync(d_run.as<uint32_t>() + S_dev, 0, size_t(S - S_dev) * 4, st));
   YD_CUDA_CHECK(cudaMemsetAsync(d_ever.as<unsigned long long>() + S_dev, 0, size_t(S - S_dev) * 8, st));
+  if (shard) {
+    d_dec.ensure(size_t(S) * 4, true, st);
+    YD_CUDA_CHECK(cudaMemsetAsync(d_dec.as<uint32_t>() + S_dev, 0, size_t(S - S_dev) * 4, st));
+  }
   S_dev = S;
 }
 
@@ -717,7 +724,7 @@ void yd_destroy(yd_sched* s) {
   cudaSetDevice(s->device);
   cudaStreamSynchronize(s->st);
   for (DevBuf* b : {&s->d_nproc, &s->d_load, &s->d_maxt, &s->d_flags, &s->d_ver, &s->d_run, &s->d_ever,
-                    &s->d_run_tmp, &s->d_ever_tmp, &s->d_remap, &s->d_env_comp, &s->d_env_local,
+                    &s->d_run_tmp, &s->d_ever_tmp, &s->d_remap, &s->d_dec, &s->d_dec_tmp, &s->d_env_comp, &s->d_env_local,
                     &s->d_comp_sv_off, &s->d_comp_sv, &s->d_comp_mask_off, &s->d_comp_nwarps, &s->d_envmask,
                     &s->d_sv_comp, &s->d_sv_local, &s->d_ip_off, &s->d_ip_sv, &s->d_ip_comp_mask, &s->d_kept_env, &s->d_kept_sv,
                     &s->d_t_exp, &s->d_t_srv,
@@ -1819,7 +1826,7 @@ void yd_free_tasks(yd_sched* s, const uint64_t* ids, size_t n) {
   YD_CUDA_CHECK(cudaMemcpyAsync(s->d_ids.p, ids, n * 8, cudaMemcpyHostToDevice, s->st));
   yd::k_free<<<(unsigned)((n + 255) / 256), 256, 0, s->st>>>(s->d_ids.as<unsigned long long>(), (uint32_t)n,
                                                               s->ring(), s->d_run.as<uint32_t>(),
-                                                              s->d_counters.as<Counters>());
+                                                              s->d_counters.as<Counters>(), s->shard ? s->d_dec.as<uint32_t>() : nullptr);
   YD_CUDA_CHECK(cudaGetLastError());
   // `ids` may be pageable and reused by the caller: the copy above has already
   // staged it (pageable H2D returns after staging) or the memory is pinned and we
@@ -1869,12 +1876,15 @@ void yd_on_expiration_timer(yd_sched* s, int64_t now_ns) {
   if (any_expired) {
     s->d_run_tmp.ensure(std::max<size_t>(size_t(S_old) * 4, 4));
     s->d_ever_tmp.ensure(std::max<size_t>(size_t(S_old) * 8, 8));
+    if (s->shard) s->d_dec_tmp.ensure(std::max<size_t>(size_t(S_old) * 4, 4));
     yd::k_compact_servants<<<(S_old + 255) / 256, 256, 0, st>>>(
         S_old, s->d_remap.as<uint32_t>(), s->d_run.as<uint32_t>(), s->d_ever.as<unsigned long long>(),
-        s->d_run_tmp.as<uint32_t>(), s->d_ever_tmp.as<unsigned long long>());
+        s->d_run_tmp.as<uint32_t>(), s->d_ever_tmp.as<unsigned long long>(), s->shard ? s->d_dec.as<uint32_t>() : nullptr,
+        s->shard ? s->d_dec_tmp.as<uint32_t>() : nullptr);
     YD_CUDA_CHECK(cudaGetLastError());
     std::swap(s->d_run, s->d_run_tmp);
     std::swap(s->d_ever, s->d_ever_tmp);
+    if (s->shard) std::swap(s->d_dec, s->d_dec_tmp);
     s->S_dev = kept;
   }
   s->FetchCounters();  // also makes `remap` (pageable) safe to drop
@@ -1932,7 +1942,8 @@ void NotifyDistinct(yd_sched* s, const yd_heartbeat_item* items, const std::vect
   if (s->zombies_ub) {
     const uint64_t cnt = s->next_id - s->lo;
     yd::k_notify_sweep<<<(unsigned)((cnt + 255) / 256), 256, 0, st>>>(s->ring(), nb, s->d_run.as<uint32_t>(),
-                                                                       s->d_counters.as<Counters>());
+                                                                       s->d_counters.as<Counters>(),
+                                                                       s->shard ? s->d_dec.as<uint32_t>() : nullptr);
     YD_CUDA_CHECK(cudaGetLastError());
   }
   if (total) {

@@ -245,8 +245,7 @@ class RangeShardedDispatcher:
 
     def wait_for_starting_new_tasks(self, reqs_local, now: float, out=None):
         """Collective.  reqs_local: this rank's FIFO range (REQ_DTYPE), or an int n = the first n staged
-        requests (TaskDispatcher.stage_requests).  Returns this rank's grants, or None if the batch has to
-        be solved on one rank (yd_shard_wait_for_starting_new_tasks returned 2: nothing was decided)."""
+        requests (TaskDispatcher.stage_requests).  Returns this rank's grants."""
         from .dispatcher import _ns
 
         lib, h = self.local._lib, self.local._h
@@ -266,8 +265,6 @@ class RangeShardedDispatcher:
         if out is None:
             out = np.zeros(max(n, 1), dtype=GRANT_DTYPE)
         rc = lib.yd_shard_wait_for_starting_new_tasks(h, _ns(now), ptr, n, out.ctypes.data)
-        if rc == 2:
-            return None
         if rc != 0:
             raise RuntimeError(f"yd_shard_wait_for_starting_new_tasks failed: {rc}")
         return out[:n]

@@ -60,6 +60,27 @@ int yd_shard_wait_for_starting_new_tasks(yd_sched* s, int64_t now_ns, const yd_t
  * that holds it and the running_tasks decrements reach every replica through one all-reduce. */
 int yd_shard_free_tasks(yd_sched* s, const uint64_t* ids, size_t n);
 
+/* STATE HANDOVER (include/ydstate.h, format version 1).  A group exports and imports as ONE scheduler: the export of
+ * a group is byte for byte what a single handle fed the concatenated queue (the same calls, the same interning)
+ * exports, and any version-1 export -- of a single handle, or of a group of any size -- imports into a group of any
+ * size, so a restart may also change the number of GPUs.  yd_export_state / yd_import_state refuse sharded handles
+ * (0 / YD_STATE_UNSUPPORTED): a lease lives on one rank, so no rank alone holds the state.
+ *
+ * Collective.  The export of the whole group.  Every rank returns the same size and, where out / cap allow, writes
+ * the same bytes (out may be NULL with cap 0 to ask for the size; that query is a collective call too).  Changes
+ * nothing: the group's later decisions are those it would have made without it.  Returns 0 on every rank if the
+ * ranks' replicated state (servants, intern tables, next task id, the bookkeeper's groups) disagrees, which is a bug
+ * and is reported on stderr. */
+size_t yd_shard_export_state(yd_sched* s, int64_t now_ns, uint8_t* out, size_t cap);
+
+/* Collective.  Loads a version-1 export into a group of fresh handles (yd_create, yd_shard_init, nothing else).
+ * Returns YD_STATE_* (ydstate.h), the SAME code on every rank.  All or nothing: if any rank refuses (not fresh, a
+ * config mismatch, no memory, a malformed blob, or a blob that differs from rank 0's: YD_STATE_BAD_BLOB), every rank
+ * returns the refusal of the lowest such rank and stays fresh.  Lease k of the export's n (ascending id order) goes
+ * to rank k * world / n; every rank's running_tasks counts every lease; a bookkeeper entry goes to the rank holding
+ * its task_grant_id's lease (rank 0 if there is none). */
+int yd_shard_import_state(yd_sched* s, int64_t now_ns, const uint8_t* blob, size_t len);
+
 /* Device time (ms, CUDA events on the solve stream) of the last sharded solve's phases: local kernels and
  * the four exchanges.  Returns 0 if there was none. */
 typedef struct yd_shard_stats {

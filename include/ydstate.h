@@ -77,14 +77,15 @@ extern "C" {
                                      * window (oldest lease to next_task_id) wider than 2^40 ids */
 #define YD_STATE_NOT_FRESH 2        /* the target handle has seen calls other than yd_create */
 #define YD_STATE_CONFIG_MISMATCH 3  /* id_stride, id_offset or the minimum memory differ from the export's */
-#define YD_STATE_UNSUPPORTED 4      /* the handle joined a range-sharded queue (include/ydshard.h) */
+#define YD_STATE_UNSUPPORTED 4      /* the handle joined a range-sharded queue: yd_shard_import_state (ydshard.h) */
 #define YD_STATE_NO_MEMORY 5        /* a valid export whose lease window does not fit the device's free memory
                                      * now (CUDA backend); the export is fine, retry when there is room */
 
 /* Serialise the handle's decision state.  Returns the byte count; writes the export to out only if
  * cap suffices (out may be NULL with cap 0 to ask for the size).  Returns 0 if the backend cannot
- * export the handle (a range-sharded handle).  Decisions after an export are those the handle would
- * have made without it. */
+ * export the handle: a range-sharded handle holds only its own leases, and its group exports together
+ * with yd_shard_export_state (ydshard.h).  Decisions after an export are those the handle would have
+ * made without it. */
 size_t yd_export_state(yd_sched* s, int64_t now_ns, uint8_t* out, size_t cap);
 
 /* Load an export into a FRESH handle (yd_create, then nothing but this call).  Returns YD_STATE_*.

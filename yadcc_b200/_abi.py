@@ -309,6 +309,8 @@ SHARD_PROTOTYPES = [
     ("yd_shard_wait_for_starting_new_tasks", C.c_int, [_P, C.c_int64, _P, C.c_size_t, _P]),
     ("yd_shard_free_tasks", C.c_int, [_P, _P, C.c_size_t]),
     ("yd_shard_last_stats", C.c_int, [_P, C.POINTER(yd_shard_stats)]),
+    ("yd_shard_export_state", C.c_size_t, [_P, C.c_int64, _P, C.c_size_t]),
+    ("yd_shard_import_state", C.c_int, [_P, C.c_int64, _P, C.c_size_t]),
 ]
 
 # Every symbol include/ydstate.h declares, and its status codes.

@@ -8,6 +8,8 @@
 //           (k_state_write), which leave the device in one copy;
 //   import  one thread per record: scatter into t_exp / t_srv / t_flags and count the lease into its
 //           servant's running_tasks (the per-servant histogram that run[] is).
+// A range-sharded group (ydshard.h) exports every rank's records, all-gathered, merged into one id order on the
+// device (k_state_merge); on import every rank counts every lease into run[] and keeps a block of them in its ring.
 #pragma once
 #include "common.cuh"
 #include "ydstate.h"
@@ -61,23 +63,50 @@ __global__ void __launch_bounds__(1024) k_state_write(TaskRing ring, long long n
   out[block_off[blockIdx.x] + before] = r;
 }
 
-// Import: records -> ring slots, and run[servant] += leases on it.  The ring's flags are zero and
-// run[] is zero before the launch.  Leases of one servant tend to sit next to each other (grants of a
-// batch), so a warp adds each distinct servant once.
-__global__ void k_state_scatter(const StateLease* __restrict__ in, uint32_t n, TaskRing ring, long long now_ns,
-                                uint32_t* __restrict__ run) {
+// Export of a range-sharded group: W record lists, list q at lists + q * stride holding counts[q] records in ascending
+// id order, disjoint (a lease lives on one rank), merged into one ascending list.  A record's place is its index in its
+// own list plus, per other list, the number of that list's ids below its own.
+__global__ void k_state_merge(const StateLease* __restrict__ lists, unsigned long long stride,
+                              const unsigned long long* __restrict__ counts, uint32_t W, StateLease* __restrict__ out) {
+  const unsigned long long t = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const uint32_t r = (uint32_t)(t / stride);
+  const unsigned long long i = t - (unsigned long long)r * stride;
+  if (r >= W || i >= counts[r]) return;
+  const StateLease rec = lists[t];
+  unsigned long long at = i;
+  for (uint32_t q = 0; q < W; ++q) {
+    if (q == r) continue;
+    const StateLease* l = lists + q * stride;
+    unsigned long long lo = 0, hi = counts[q];
+    while (lo < hi) {
+      const unsigned long long mid = (lo + hi) >> 1;
+      if (l[mid].id < rec.id) lo = mid + 1; else hi = mid;
+    }
+    at += lo;
+  }
+  out[at] = rec;
+}
+
+// Import: records -> ring slots, and run[servant] += leases on it.  Every record counts into run[]; only records
+// [keep_lo, keep_hi) enter the ring (all of them on a single handle, this rank's block on a range-sharded one).  The
+// ring's flags are zero and run[] is zero before the launch.  Leases of one servant tend to sit next to each other
+// (grants of a batch), so a warp adds each distinct servant once.
+__global__ void k_state_scatter(const StateLease* __restrict__ in, uint32_t n, uint32_t keep_lo, uint32_t keep_hi,
+                                TaskRing ring, long long now_ns, uint32_t* __restrict__ run) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   const bool have = i < n;
   uint32_t servant = kNone;
   if (have) {
     const StateLease r = in[i];
-    unsigned long long local = 0;
-    ring.loc(r.id, &local);  // (the host checked that every id is one of ours)
-    const uint64_t slot = local & ring.mask;
-    ring.exp[slot] = now_ns + r.expires_rel;
-    ring.srv[slot] = r.servant;
-    ring.flags[slot] = kTaskAlive | ((r.flags & YD_STATE_LEASE_PREFETCH) ? kTaskPrefetch : 0u) |
-                       ((r.flags & YD_STATE_LEASE_ZOMBIE) ? kTaskZombie : 0u);
+    if (i >= keep_lo && i < keep_hi) {
+      unsigned long long local = 0;
+      ring.loc(r.id, &local);  // (the host checked that every id is one of ours)
+      const uint64_t slot = local & ring.mask;
+      ring.exp[slot] = now_ns + r.expires_rel;
+      ring.srv[slot] = r.servant;
+      ring.flags[slot] = kTaskAlive | ((r.flags & YD_STATE_LEASE_PREFETCH) ? kTaskPrefetch : 0u) |
+                         ((r.flags & YD_STATE_LEASE_ZOMBIE) ? kTaskZombie : 0u);
+    }
     servant = r.servant;
   }
   const uint32_t peers = __match_any_sync(0xffffffffu, servant);

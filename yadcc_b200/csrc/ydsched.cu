@@ -137,6 +137,9 @@ struct ServantHost {  // ServantPersonality + ServantDesc lease fields (h:80-116
 struct RunningRec {
   uint64_t servant_task_id, task_grant_id;
   std::string servant_location, task_digest;
+  // Index of the task in the heartbeat that reported it.  A rank of a range-sharded queue keeps only the reported tasks
+  // whose lease it holds; the ranks' groups merged by this index are the single scheduler's (yd_shard_export_state).
+  uint32_t report_pos = 0;
 };
 
 // The sequence of a slot-stream solve (EnqueueSolve); the YDSCHED_DEBUG line prints the number.
@@ -2000,7 +2003,7 @@ size_t yd_notify_servants_running_tasks(yd_sched* s, const yd_heartbeat_item* it
         } else {
           kept.push_back(RunningRec{it.tasks[t].servant_task_id, it.tasks[t].task_grant_id,
                                     it.tasks[t].servant_location ? it.tasks[t].servant_location : "",
-                                    it.tasks[t].task_digest ? it.tasks[t].task_digest : ""});
+                                    it.tasks[t].task_digest ? it.tasks[t].task_digest : "", (uint32_t)t});
         }
       }
       // RunningTaskBookkeeper::SetServantRunningTasks, running_task_bookkeeper.cc:24-29
@@ -2554,34 +2557,49 @@ void* StateTmp(yd_sched* s, size_t bytes) {
 
 }  // namespace
 
-extern "C" size_t yd_export_state(yd_sched* s, int64_t now_ns, uint8_t* out, size_t cap) {
-  if (s->shard) return 0;  // range-sharded handles are not exported
-  YD_CUDA_CHECK(cudaSetDevice(s->device));
-  cudaStream_t st = s->st;
-  s->SyncServantState();
-  const size_t S = s->sv.size();
-  // ever_assigned_tasks of every servant and the live-lease count of the window, one synchronisation
-  std::vector<unsigned long long> ever(S);
-  if (S) YD_CUDA_CHECK(cudaMemcpyAsync(ever.data(), s->d_ever.p, S * 8, cudaMemcpyDeviceToHost, st));
-  const uint64_t window = s->next_id - s->lo;
-  const uint32_t nb = (uint32_t)((window + 1023) / 1024);
+namespace {
+
+// The live leases of the ring's window: per 1024-id block a count, scanned (k_state_count + k_final_scan).  `n` is
+// valid after the stream's next synchronisation; the scratch goes with FreeLiveLeases.
+struct LiveLeases {
+  uint32_t nb = 0;
   uint32_t* d_off = nullptr;
   Counters* d_sum = nullptr;
-  unsigned long long n_leases = 0;
-  if (nb) {
-    char* t = static_cast<char*>(StateTmp(s, sizeof(Counters) + size_t(nb) * 4));
-    d_sum = reinterpret_cast<Counters*>(t);
-    d_off = reinterpret_cast<uint32_t*>(t + sizeof(Counters));
-    YD_CUDA_CHECK(cudaMemsetAsync(d_sum, 0, sizeof(Counters), st));
-    yd::k_state_count<<<nb, 1024, 0, st>>>(s->ring(), d_off);
-    YD_CUDA_CHECK(cudaGetLastError());
-    // the exclusive scan of the grant path, into a scratch Counters (its total lands in ->granted)
-    yd::k_final_scan<<<1, 1024, 0, st>>>(d_off, nb, d_sum, nullptr);
-    YD_CUDA_CHECK(cudaGetLastError());
-    YD_CUDA_CHECK(cudaMemcpyAsync(&n_leases, &d_sum->granted, 8, cudaMemcpyDeviceToHost, st));
-  }
-  YD_CUDA_CHECK(cudaStreamSynchronize(st));
+  unsigned long long n = 0;
+};
 
+void CountLiveLeases(yd_sched* s, LiveLeases* L) {
+  cudaStream_t st = s->st;
+  L->nb = (uint32_t)((s->next_id - s->lo + 1023) / 1024);
+  if (!L->nb) return;
+  char* t = static_cast<char*>(StateTmp(s, sizeof(Counters) + size_t(L->nb) * 4));
+  L->d_sum = reinterpret_cast<Counters*>(t);
+  L->d_off = reinterpret_cast<uint32_t*>(t + sizeof(Counters));
+  YD_CUDA_CHECK(cudaMemsetAsync(L->d_sum, 0, sizeof(Counters), st));
+  yd::k_state_count<<<L->nb, 1024, 0, st>>>(s->ring(), L->d_off);
+  YD_CUDA_CHECK(cudaGetLastError());
+  // the exclusive scan of the grant path, into a scratch Counters (its total lands in ->granted)
+  yd::k_final_scan<<<1, 1024, 0, st>>>(L->d_off, L->nb, L->d_sum, nullptr);
+  YD_CUDA_CHECK(cudaGetLastError());
+  YD_CUDA_CHECK(cudaMemcpyAsync(&L->n, &L->d_sum->granted, 8, cudaMemcpyDeviceToHost, st));
+}
+
+// The counted leases as records, in id order, at d_rec.
+void WriteLiveLeases(yd_sched* s, const LiveLeases& L, int64_t now_ns, yd::StateLease* d_rec) {
+  yd::k_state_write<<<L.nb, 1024, 0, s->st>>>(s->ring(), (long long)now_ns, L.d_off, d_rec);
+  YD_CUDA_CHECK(cudaGetLastError());
+}
+
+void FreeLiveLeases(yd_sched* s, const LiveLeases& L) {
+  if (L.d_sum) YD_CUDA_CHECK(cudaFreeAsync(L.d_sum, s->st));
+}
+
+// Every section of the export but the lease records (n_leases stays 0).  Synchronises the stream.
+ydstate::StateImage HostImage(yd_sched* s, int64_t now_ns) {
+  const size_t S = s->sv.size();
+  std::vector<unsigned long long> ever(S);
+  if (S) YD_CUDA_CHECK(cudaMemcpyAsync(ever.data(), s->d_ever.p, S * 8, cudaMemcpyDeviceToHost, s->st));
+  YD_CUDA_CHECK(cudaStreamSynchronize(s->st));
   ydstate::StateImage im;
   im.id_stride = s->id_stride;
   im.id_offset = s->id_offset;
@@ -2602,45 +2620,61 @@ extern "C" size_t yd_export_state(yd_sched* s, int64_t now_ns, uint8_t* out, siz
     o.envs.reserve(v.envs.size());
     for (uint32_t e : v.envs) o.envs.push_back(s->envs[e]);
   }
-  im.n_leases = n_leases;  // (written straight into `out` below)
   im.bucket_count = s->running.bucket_count();
   for (auto&& [loc, v] : s->running) {
     ydstate::Group& g = im.groups.emplace_back();
     g.location = loc;
     for (auto&& t : v) g.tasks.push_back(ydstate::Task{t.servant_task_id, t.task_grant_id, t.servant_location, t.task_digest});
   }
-  size_t lease_off = 0;
-  const size_t size = ydstate::EncodeState(im, out, cap, &lease_off);
-  if (out && cap >= size && n_leases) {
-    yd::StateLease* d_rec = static_cast<yd::StateLease*>(StateTmp(s, n_leases * sizeof(yd::StateLease)));
-    yd::k_state_write<<<nb, 1024, 0, st>>>(s->ring(), (long long)now_ns, d_off, d_rec);
-    YD_CUDA_CHECK(cudaGetLastError());
-    YD_CUDA_CHECK(cudaMemcpyAsync(out + lease_off, d_rec, n_leases * sizeof(yd::StateLease), cudaMemcpyDeviceToHost, st));
-    YD_CUDA_CHECK(cudaFreeAsync(d_rec, st));
-  }
-  if (d_sum) YD_CUDA_CHECK(cudaFreeAsync(d_sum, st));
-  YD_CUDA_CHECK(cudaStreamSynchronize(st));
-  return size;
+  return im;
 }
 
-extern "C" int yd_import_state(yd_sched* s, int64_t now_ns, const uint8_t* blob, size_t len) {
-  if (s->shard) return YD_STATE_UNSUPPORTED;
+// The leases [*k0, *k1) (ascending id order) that rank `rank` of `world` holds after an import: lease k of n goes to
+// rank k * world / n, contiguous id blocks.  One rank holds all of them.
+void HeldBlock(uint64_t n, uint32_t rank, uint32_t world, uint64_t* k0, uint64_t* k1) {
+  *k0 = (uint64_t(rank) * n + world - 1) / world;
+  *k1 = (uint64_t(rank + 1) * n + world - 1) / world;
+}
+
+uint32_t LeaseHolder(const ydstate::StateImage& im, uint64_t task_grant_id, uint32_t world) {
+  const auto& L = im.leases;
+  auto it = std::lower_bound(L.begin(), L.end(), task_grant_id, [](const ydstate::Lease& l, uint64_t id) { return l.id < id; });
+  if (it == L.end() || it->id != task_grant_id) return 0;  // a bookkeeper entry whose lease is gone: rank 0 keeps it
+  return (uint32_t)(uint64_t(it - L.begin()) * world / L.size());
+}
+
+// Everything an import can refuse, checked before anything changes: freshness, the blob, the config, and room on the
+// device for the ring of the leases this rank will hold.
+int CheckImport(yd_sched* s, const uint8_t* blob, size_t len, uint32_t rank, uint32_t world, ydstate::StateImage* im) {
   if (!IsFresh(s)) return YD_STATE_NOT_FRESH;
-  ydstate::StateImage im;
-  if (int rc = ydstate::DecodeState(blob, len, &im)) return rc;
-  if (im.id_stride != s->id_stride || im.id_offset != s->id_offset || im.min_mem != s->min_mem) return YD_STATE_CONFIG_MISMATCH;
+  if (int rc = ydstate::DecodeState(blob, len, im)) return rc;
+  if (im->id_stride != s->id_stride || im->id_offset != s->id_offset || im->min_mem != s->min_mem) return YD_STATE_CONFIG_MISMATCH;
   YD_CUDA_CHECK(cudaSetDevice(s->device));
-  cudaStream_t st = s->st;
-  auto local = [&](uint64_t ext) { return (ext - im.id_offset) / im.id_stride; };
-  const uint64_t next_id = local(im.next_task_id);
-  const uint64_t lo = im.leases.empty() ? next_id : local(im.leases.front().id);
+  auto local = [&](uint64_t ext) { return (ext - im->id_offset) / im->id_stride; };
+  uint64_t k0, k1;
+  HeldBlock(im->leases.size(), rank, world, &k0, &k1);
+  const uint64_t next_id = local(im->next_task_id);
+  const uint64_t lo = k0 < k1 ? local(im->leases[k0].id) : next_id;
   // The ring is sized from the oldest live id, as EnsureRing would have grown it (DecodeState bounds the window by
   // kMaxWindow, so none of this overflows); a valid export that cannot fit the device's free memory now is refused.
   uint64_t ring_cap = 1ull << 16;
   while (ring_cap < (next_id - lo) * 2) ring_cap <<= 1;
   size_t free_b = 0, total_b = 0;
   YD_CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
-  if (ring_cap * 16 + im.leases.size() * sizeof(yd::StateLease) > free_b) return YD_STATE_NO_MEMORY;
+  if (ring_cap * 16 + im->leases.size() * sizeof(yd::StateLease) > free_b) return YD_STATE_NO_MEMORY;
+  return YD_STATE_OK;
+}
+
+// Loads a checked image: the replicated state in full, the leases rank `rank` of `world` holds into the ring, every
+// lease into running_tasks, and the bookkeeper entries whose lease the rank holds.
+void ApplyImport(yd_sched* s, int64_t now_ns, const ydstate::StateImage& im, uint32_t rank, uint32_t world) {
+  cudaStream_t st = s->st;
+  auto local = [&](uint64_t ext) { return (ext - im.id_offset) / im.id_stride; };
+  const size_t n = im.leases.size();
+  uint64_t k0, k1;
+  HeldBlock(n, rank, world, &k0, &k1);
+  const uint64_t next_id = local(im.next_task_id);
+  const uint64_t lo = k0 < k1 ? local(im.leases[k0].id) : next_id;
 
   // host side: exactly what KeepServantAlive, the interning calls and the bookkeeper would have built
   s->envs = im.envs;
@@ -2664,11 +2698,16 @@ extern "C" int yd_import_state(yd_sched* s, int64_t now_ns, const uint8_t* blob,
     s->loc2pos.emplace(rec.observed, i);
     ever[i] = v.ever;
   }
-  // the bookkeeper's iteration order: same bucket count, groups inserted last-first (ydstate.h)
+  // the bookkeeper's iteration order: same bucket count, groups inserted last-first (ydstate.h); every rank has every
+  // group, as every rank sees every heartbeat
   if (im.bucket_count != 1) s->running.rehash(im.bucket_count);
   for (auto g = im.groups.rbegin(); g != im.groups.rend(); ++g) {
     std::vector<RunningRec> v;
-    for (auto&& t : g->tasks) v.push_back(RunningRec{t.servant_task_id, t.task_grant_id, t.servant_location, t.task_digest});
+    for (uint32_t j = 0; j != g->tasks.size(); ++j) {
+      const ydstate::Task& t = g->tasks[j];
+      if (world == 1 || LeaseHolder(im, t.task_grant_id, world) == rank)
+        v.push_back(RunningRec{t.servant_task_id, t.task_grant_id, t.servant_location, t.task_digest, j});
+    }
     s->running.emplace(g->location, std::move(v));
   }
   s->topo_dirty = s->facts_dirty = s->order_dirty = true;  // the first solve rebuilds topology, facts and slot order
@@ -2679,6 +2718,10 @@ extern "C" int yd_import_state(yd_sched* s, int64_t now_ns, const uint8_t* blob,
     s->d_ever.ensure(size_t(S) * 8);
     YD_CUDA_CHECK(cudaMemsetAsync(s->d_run.p, 0, size_t(S) * 4, st));
     YD_CUDA_CHECK(cudaMemcpyAsync(s->d_ever.p, ever.data(), size_t(S) * 8, cudaMemcpyHostToDevice, st));
+    if (s->shard) {  // every rank's running_tasks is the whole group's: nothing to hand to the others
+      s->d_dec.ensure(size_t(S) * 4);
+      YD_CUDA_CHECK(cudaMemsetAsync(s->d_dec.p, 0, size_t(S) * 4, st));
+    }
   }
   s->S_dev = S;
   s->d_t_exp.release(); s->d_t_srv.release(); s->d_t_flags.release();
@@ -2686,24 +2729,227 @@ extern "C" int yd_import_state(yd_sched* s, int64_t now_ns, const uint8_t* blob,
   s->lo = lo;
   s->next_id = next_id;
   s->EnsureRing(0);
-  const size_t n = im.leases.size();
   uint64_t zombies = 0;
-  for (auto&& l : im.leases) zombies += (l.flags & YD_STATE_LEASE_ZOMBIE) != 0;
+  for (uint64_t k = k0; k < k1; ++k) zombies += (im.leases[k].flags & YD_STATE_LEASE_ZOMBIE) != 0;
   if (n) {
     yd::StateLease* d_rec = static_cast<yd::StateLease*>(StateTmp(s, n * sizeof(yd::StateLease)));
     YD_CUDA_CHECK(cudaMemcpyAsync(d_rec, im.leases.data(), n * sizeof(yd::StateLease), cudaMemcpyHostToDevice, st));
-    yd::k_state_scatter<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_rec, (uint32_t)n, s->ring(), (long long)now_ns,
-                                                                    s->d_run.as<uint32_t>());
+    yd::k_state_scatter<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_rec, (uint32_t)n, (uint32_t)k0, (uint32_t)k1, s->ring(),
+                                                                    (long long)now_ns, s->d_run.as<uint32_t>());
     YD_CUDA_CHECK(cudaGetLastError());
     YD_CUDA_CHECK(cudaFreeAsync(d_rec, st));
   }
   Counters* c = s->h_counters.as<Counters>();
   memset(c, 0, sizeof(Counters));
-  c->alive = n;
+  c->alive = k1 - k0;
   c->zombies = zombies;
   c->min_live = ~0ull;
   YD_CUDA_CHECK(cudaMemcpyAsync(s->d_counters.p, c, sizeof(Counters), cudaMemcpyHostToDevice, st));
   YD_CUDA_CHECK(cudaStreamSynchronize(st));
   s->zombies_ub = zombies;
+}
+
+}  // namespace
+
+extern "C" size_t yd_export_state(yd_sched* s, int64_t now_ns, uint8_t* out, size_t cap) {
+  if (s->shard) return 0;  // a range-sharded handle holds part of the leases: yd_shard_export_state
+  YD_CUDA_CHECK(cudaSetDevice(s->device));
+  cudaStream_t st = s->st;
+  s->SyncServantState();
+  LiveLeases L;
+  CountLiveLeases(s, &L);
+  ydstate::StateImage im = HostImage(s, now_ns);
+  im.n_leases = L.n;  // (written straight into `out` below)
+  size_t lease_off = 0;
+  const size_t size = ydstate::EncodeState(im, out, cap, &lease_off);
+  if (out && cap >= size && L.n) {
+    yd::StateLease* d_rec = static_cast<yd::StateLease*>(StateTmp(s, L.n * sizeof(yd::StateLease)));
+    WriteLiveLeases(s, L, now_ns, d_rec);
+    YD_CUDA_CHECK(cudaMemcpyAsync(out + lease_off, d_rec, L.n * sizeof(yd::StateLease), cudaMemcpyDeviceToHost, st));
+    YD_CUDA_CHECK(cudaFreeAsync(d_rec, st));
+  }
+  FreeLiveLeases(s, L);
+  YD_CUDA_CHECK(cudaStreamSynchronize(st));
+  return size;
+}
+
+extern "C" int yd_import_state(yd_sched* s, int64_t now_ns, const uint8_t* blob, size_t len) {
+  if (s->shard) return YD_STATE_UNSUPPORTED;  // yd_shard_import_state
+  ydstate::StateImage im;
+  if (int rc = CheckImport(s, blob, len, 0, 1, &im)) return rc;
+  ApplyImport(s, now_ns, im, 0, 1);
+  return YD_STATE_OK;
+}
+
+// ---- state export / import of a range-sharded group (ydshard.h) --------------------------------------------------------
+// The replicated sections come from each rank's own image (checked equal through a hash); the leases and the
+// bookkeeper's tasks, which each live on one rank, are gathered and merged.
+namespace {
+
+uint64_t Fnv1a(const uint8_t* p, size_t n) {
+  uint64_t h = 0xcbf29ce484222325ull;
+  for (size_t i = 0; i != n; ++i) h = (h ^ p[i]) * 0x100000001b3ull;
+  return h;
+}
+
+// All-gather of `mine` (the same word count on every rank) through device scratch: every rank's words, rank-major.
+std::vector<uint32_t> GatherWords(yd_sched* s, const std::vector<uint32_t>& mine) {
+  yd_shard_ctx* c = s->shard;
+  const size_t W = (size_t)c->world, words = mine.size();
+  uint32_t* d = static_cast<uint32_t*>(StateTmp(s, words * 4 * (W + 1)));
+  YD_CUDA_CHECK(cudaMemcpyAsync(d, mine.data(), words * 4, cudaMemcpyHostToDevice, s->st));
+  YD_NCCL_CHECK(c->api, c->api->AllGather(d, d + words, words, ncclUint32, c->comm, s->st));
+  std::vector<uint32_t> all(words * W);
+  YD_CUDA_CHECK(cudaMemcpyAsync(all.data(), d + words, words * 4 * W, cudaMemcpyDeviceToHost, s->st));
+  YD_CUDA_CHECK(cudaFreeAsync(d, s->st));
+  YD_CUDA_CHECK(cudaStreamSynchronize(s->st));
+  return all;
+}
+
+void PutU64(std::vector<uint32_t>& v, uint64_t x) { v.push_back((uint32_t)x); v.push_back((uint32_t)(x >> 32)); }
+uint64_t GetU64(const uint32_t* p) { return p[0] | (uint64_t(p[1]) << 32); }
+
+// This rank's bookkeeper tasks, group by group in iteration order: u32 count, then per task its report position,
+// servant_task_id, task_grant_id and the two strings (u32 byte length, bytes), packed into u32 words.
+std::vector<uint32_t> PackBook(const yd_sched* s) {
+  std::string b;
+  auto put = [&](const void* p, size_t n) { b.append(static_cast<const char*>(p), n); };
+  auto str = [&](const std::string& x) { const uint32_t n = (uint32_t)x.size(); put(&n, 4); put(x.data(), n); };
+  for (auto&& [loc, v] : s->running) {
+    const uint32_t n = (uint32_t)v.size();
+    put(&n, 4);
+    for (auto&& t : v) {
+      put(&t.report_pos, 4); put(&t.servant_task_id, 8); put(&t.task_grant_id, 8);
+      str(t.servant_location); str(t.task_digest);
+    }
+  }
+  std::vector<uint32_t> w((b.size() + 3) / 4, 0);
+  if (!b.empty()) memcpy(w.data(), b.data(), b.size());
+  return w;
+}
+
+// The groups' tasks of every rank's packed book (W blocks of `stride` words), merged by report position.
+void MergeBooks(const std::vector<uint32_t>& all, size_t stride, uint32_t W, std::vector<ydstate::Group>* groups) {
+  std::vector<std::vector<std::pair<uint32_t, ydstate::Task>>> got(groups->size());
+  for (uint32_t r = 0; r < W; ++r) {
+    const char* p = reinterpret_cast<const char*>(all.data() + r * stride);
+    auto get = [&](void* o, size_t n) { memcpy(o, p, n); p += n; };
+    auto str = [&]() { uint32_t n; get(&n, 4); std::string x(p, n); p += n; return x; };
+    for (auto& g : got) {
+      uint32_t n;
+      get(&n, 4);
+      for (uint32_t k = 0; k != n; ++k) {
+        uint32_t pos;
+        ydstate::Task t;
+        get(&pos, 4); get(&t.servant_task_id, 8); get(&t.task_grant_id, 8);
+        t.servant_location = str();
+        t.task_digest = str();
+        g.emplace_back(pos, std::move(t));
+      }
+    }
+  }
+  for (size_t i = 0; i != got.size(); ++i) {
+    std::sort(got[i].begin(), got[i].end(), [](auto& a, auto& b) { return a.first < b.first; });
+    auto& tasks = (*groups)[i].tasks;
+    tasks.clear();
+    for (auto& pt : got[i]) tasks.push_back(std::move(pt.second));
+  }
+}
+
+}  // namespace
+
+extern "C" size_t yd_shard_export_state(yd_sched* s, int64_t now_ns, uint8_t* out, size_t cap) {
+  yd_shard_ctx* c = s ? s->shard : nullptr;
+  if (!c) return 0;
+  YD_CUDA_CHECK(cudaSetDevice(s->device));
+  cudaStream_t st = s->st;
+  const uint32_t W = (uint32_t)c->world;
+  s->SyncServantState();
+  LiveLeases L;
+  CountLiveLeases(s, &L);
+  ydstate::StateImage im = HostImage(s, now_ns);
+  // the replicated sections: the image without lease records and without the groups' tasks
+  std::vector<ydstate::Group> groups = std::move(im.groups);
+  im.groups.clear();
+  for (auto&& g : groups) im.groups.push_back(ydstate::Group{g.location, {}});
+  std::vector<uint8_t> rep(ydstate::EncodeState(im, nullptr, 0));
+  ydstate::EncodeState(im, rep.data(), rep.size());
+  const std::vector<uint32_t> book = PackBook(s);
+  // exchange 1: lease count, hash of the replicated sections, packed book length, the room this rank offers
+  std::vector<uint32_t> hdr;
+  PutU64(hdr, L.n);
+  PutU64(hdr, Fnv1a(rep.data(), rep.size()));
+  PutU64(hdr, book.size());
+  PutU64(hdr, out ? cap : 0);
+  const std::vector<uint32_t> all = GatherWords(s, hdr);
+  std::vector<unsigned long long> counts(W);
+  uint64_t n_total = 0, maxn = 0, maxbook = 0;
+  for (uint32_t r = 0; r < W; ++r) {
+    const uint32_t* h = all.data() + r * hdr.size();
+    counts[r] = GetU64(h);
+    n_total += counts[r];
+    maxn = std::max<uint64_t>(maxn, counts[r]);
+    maxbook = std::max<uint64_t>(maxbook, GetU64(h + 4));
+    if (GetU64(h + 2) != GetU64(all.data() + 2)) {
+      fprintf(stderr, "ydsched: yd_shard_export_state: rank %u's replicated state differs from rank 0's\n", r);
+      FreeLiveLeases(s, L);
+      YD_CUDA_CHECK(cudaStreamSynchronize(st));
+      return 0;
+    }
+  }
+  // exchange 2: the books, padded to the longest
+  if (maxbook) {
+    std::vector<uint32_t> mine = book;
+    mine.resize(maxbook, 0);
+    MergeBooks(GatherWords(s, mine), maxbook, W, &groups);
+  }
+  im.groups = std::move(groups);
+  im.n_leases = n_total;
+  size_t lease_off = 0;
+  const size_t size = ydstate::EncodeState(im, nullptr, 0, &lease_off);
+  bool any_room = false;
+  for (uint32_t r = 0; r < W; ++r) any_room |= GetU64(all.data() + r * hdr.size() + 6) >= size;
+  const bool write = out && cap >= size;
+  if (write) ydstate::EncodeState(im, out, cap);
+  // exchange 3 (when some rank writes the export): the lease records, padded to the longest list, merged on the device
+  if (any_room && n_total) {
+    const size_t rb = sizeof(yd::StateLease);
+    char* t = static_cast<char*>(StateTmp(s, maxn * rb * (W + 1) + n_total * rb + W * 8));
+    yd::StateLease* d_send = reinterpret_cast<yd::StateLease*>(t);
+    yd::StateLease* d_lists = d_send + maxn;
+    yd::StateLease* d_out = d_lists + maxn * W;
+    unsigned long long* d_counts = reinterpret_cast<unsigned long long*>(d_out + n_total);
+    if (L.n) WriteLiveLeases(s, L, now_ns, d_send);
+    YD_CUDA_CHECK(cudaMemcpyAsync(d_counts, counts.data(), W * 8, cudaMemcpyHostToDevice, st));
+    YD_NCCL_CHECK(c->api, c->api->AllGather(d_send, d_lists, maxn * rb / 4, ncclUint32, c->comm, st));
+    const uint64_t threads = maxn * W;
+    yd::k_state_merge<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(d_lists, maxn, d_counts, W, d_out);
+    YD_CUDA_CHECK(cudaGetLastError());
+    if (write) YD_CUDA_CHECK(cudaMemcpyAsync(out + lease_off, d_out, n_total * rb, cudaMemcpyDeviceToHost, st));
+    YD_CUDA_CHECK(cudaFreeAsync(t, st));
+  }
+  FreeLiveLeases(s, L);
+  YD_CUDA_CHECK(cudaStreamSynchronize(st));
+  return size;
+}
+
+extern "C" int yd_shard_import_state(yd_sched* s, int64_t now_ns, const uint8_t* blob, size_t len) {
+  yd_shard_ctx* c = s ? s->shard : nullptr;
+  if (!c) return YD_STATE_UNSUPPORTED;
+  YD_CUDA_CHECK(cudaSetDevice(s->device));
+  const uint32_t W = (uint32_t)c->world, R = (uint32_t)c->rank;
+  ydstate::StateImage im;
+  const int rc = CheckImport(s, blob, len, R, W, &im);
+  // every rank's verdict and the length and hash of its blob: all or nothing, and only rank 0's export is loaded
+  std::vector<uint32_t> mine{(uint32_t)rc, 0};
+  PutU64(mine, len);
+  PutU64(mine, blob ? Fnv1a(blob, len) : 0);
+  const std::vector<uint32_t> all = GatherWords(s, mine);
+  for (uint32_t r = 0; r < W; ++r) {
+    const uint32_t* v = all.data() + r * mine.size();
+    if (v[0] != YD_STATE_OK) return (int)v[0];
+    if (GetU64(v + 2) != GetU64(all.data() + 2) || GetU64(v + 4) != GetU64(all.data() + 4)) return YD_STATE_BAD_BLOB;
+  }
+  ApplyImport(s, now_ns, im, R, W);
   return YD_STATE_OK;
 }

@@ -77,7 +77,7 @@ class StateError(RuntimeError):
     """yd_import_state refused an export; `code` is one of _abi.STATE_* (ydstate.h)."""
 
     NAMES = {1: "malformed export", 2: "the handle is not fresh", 3: "the export's config differs from the handle's",
-             4: "range-sharded handles have no state export",
+             4: "a range-sharded handle: its group exports and imports together (RangeShardedDispatcher)",
              5: "the export's lease window does not fit the device's free memory now"}
 
     def __init__(self, code: int):
@@ -168,6 +168,10 @@ class TaskDispatcher:
         id_offset: int = 0,
     ):
         self._lib = library if isinstance(library, C.CDLL) else _abi.load_library(library)
+        # (a handle of the same backend and config: RangeShardedDispatcher.import_state checks an export on one)
+        self._config = dict(device=device, servant_min_memory_for_accepting_new_task=servant_min_memory_for_accepting_new_task,
+                            solver=solver, graphs=graphs, merge_self=merge_self, tiny=tiny, fused=fused,
+                            id_stride=id_stride, id_offset=id_offset)
         cfg = _abi.yd_config(
             abi_version=_abi.ABI_VERSION,
             device=device,

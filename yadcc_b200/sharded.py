@@ -283,6 +283,66 @@ class RangeShardedDispatcher:
         if rc != 0:
             raise RuntimeError(f"yd_shard_free_tasks failed: {rc}")
 
+    def export_state(self, now: float = 0.0) -> bytes:
+        """Collective.  The group's state as ONE scheduler's export (ydstate.h), the same bytes on every rank: a
+        single TaskDispatcher, or a group of any size, can import it (import_state)."""
+        import ctypes as C
+
+        from .dispatcher import _ns
+
+        if not self.native:
+            return self.local.export_state(now)  # every replica holds every lease
+        lib, h, t = self.local._lib, self.local._h, _ns(now)
+        n = lib.yd_shard_export_state(h, t, None, 0)
+        if n == 0:
+            raise RuntimeError("yd_shard_export_state: the ranks' replicated state disagrees")
+        buf = C.create_string_buffer(n)
+        m = lib.yd_shard_export_state(h, t, buf, n)
+        assert m == n, (m, n)
+        return buf.raw
+
+    def import_state(self, blob: bytes, now: float = 0.0) -> None:
+        """Collective.  Load an export (of a single handle or of a group of any size) into this group of fresh
+        handles.  All or nothing: if any rank refuses, every rank raises StateError with the same code and stays
+        fresh."""
+        from . import _abi
+        from .dispatcher import StateError, TaskDispatcher, _ns
+
+        data = bytes(blob)
+        if self.native:
+            rc = self.local._lib.yd_shard_import_state(self.local._h, _ns(now), data, len(data))
+            if rc != _abi.STATE_OK:
+                raise StateError(rc)
+            return
+        import hashlib
+
+        import torch.distributed as dist
+
+        # Every refusal leaves a handle fresh, but a success does not: check on a scratch handle of the same library
+        # and config first, so that the local import runs only where every rank will succeed.  An empty blob is
+        # refused as not fresh, or as malformed by a fresh handle.
+        rc = _abi.STATE_OK
+        try:
+            self.local.import_state(b"", now)
+        except StateError as e:
+            rc = e.code if e.code == _abi.STATE_NOT_FRESH else _abi.STATE_OK
+        if rc == _abi.STATE_OK:
+            scratch = TaskDispatcher(self.local._lib, **self.local._config)
+            try:
+                scratch.import_state(data, now)
+            except StateError as e:
+                rc = e.code
+            finally:
+                scratch.close()
+        verdicts: list = [None] * self.world
+        dist.all_gather_object(verdicts, (rc, hashlib.sha256(data).digest()), group=self.group)
+        for code, digest in verdicts:
+            if code == _abi.STATE_OK and digest != verdicts[0][1]:
+                code = _abi.STATE_BAD_BLOB
+            if code != _abi.STATE_OK:
+                raise StateError(code)
+        self.local.import_state(data, now)
+
     def last_stats(self) -> dict | None:
         import ctypes as C
 

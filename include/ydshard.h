@@ -28,6 +28,7 @@
 #define YDSHARD_H_
 
 #include "ydsched.h"
+#include "ydservice.h"
 
 #ifdef __cplusplus
 extern "C" {
@@ -80,6 +81,49 @@ size_t yd_shard_export_state(yd_sched* s, int64_t now_ns, uint8_t* out, size_t c
  * to rank k * world / n; every rank's running_tasks counts every lease; a bookkeeper entry goes to the rank holding
  * its task_grant_id's lease (rank 0 if there is none). */
 int yd_shard_import_state(yd_sched* s, int64_t now_ns, const uint8_t* blob, size_t len);
+
+/* REPLICATED CALLS: the rest of TaskDispatcher, and SchedulerServiceImpl, answered by the group as ONE scheduler.
+ * Every rank makes the call with the same arguments, in the same order relative to the other calls on its handle (the
+ * conditions under which a front end feeds every rank the same heartbeats); every rank then returns the same answer,
+ * and it is what one handle fed the concatenated queue returns for the same call.  Arguments are not checked across
+ * ranks: ranks that pass different ones get answers that match no single scheduler.  Each call makes one exchange
+ * (GetRunningTasks two, WaitForStartingTask one more than its solve) and the running_tasks decrements a rank has not
+ * shared yet ride along it, so the invariant above holds after each.  On a handle that has not joined a group, the
+ * calls that return a count are the single-handle call.  The per-rank calls of ydsched.h (yd_keep_task_alive,
+ * yd_notify_*, yd_get_running_tasks, yd_running_index_refresh, yd_wait_for_starting_task_rpcs) keep answering for the
+ * rank's own leases only.
+ *
+ * KeepTaskAlive x n.  The holder of a lease renews it, the other ranks answer 0; one sum all-reduce of a u32 flag per
+ * id and the decrements.  Returns 0; 1 (nothing exchanged) if the handle has not joined a group or n >= 2^30. */
+int yd_shard_keep_task_alive(yd_sched* s, int64_t now_ns, const uint64_t* task_ids, size_t n, int64_t new_expires_in_ns,
+                             uint8_t* ok_out);
+/* NotifyServantRunningTasks x n, as yd_notify_servants_running_tasks.  Each rank sweeps and checks its own leases; one
+ * sum all-reduce of a u32 word per reported id (rank + 1 where permitted) and the decrements.  An id is unknown iff no
+ * rank permits it.  Each rank's bookkeeper keeps the tasks whose lease it holds. */
+size_t yd_shard_notify_servants_running_tasks(yd_sched* s, const yd_heartbeat_item* items, size_t n, uint64_t* unknown_out,
+                                              size_t* unknown_counts);
+/* GetRunningTasks, in the single scheduler's order.  Two all-gathers: the packed bookkeepers' lengths with the
+ * decrements, then the bookkeepers, merged by each task's position in the heartbeat that reported it.  The strings stay
+ * valid until the next call that mutates the handle. */
+size_t yd_shard_get_running_tasks(yd_sched* s, yd_running_task* out, size_t cap);
+/* RunningTaskKeeper::Refresh over the group: the snapshot is yd_shard_get_running_tasks' list, so yd_running_index_find
+ * and yd_running_index_entry on any rank then answer for the whole group. */
+size_t yd_shard_running_index_refresh(yd_sched* s);
+/* WaitForStartingTask x n_rpcs, as yd_wait_for_starting_task_rpcs (the same expansion, limits and return values).  The
+ * expanded queue is cut into `world` even contiguous ranges; each rank expands its own and decides it with
+ * yd_shard_wait_for_starting_new_tasks, and one all-gather (a grant is 4 u32 words, padded to the longest range) gives
+ * every rank the whole window's decisions, to which it applies the stop rules.  A refusal ((size_t)-1: cap too small, a
+ * batch above 2^30 decisions, or capacities above 8192 per servant) happens on every rank and decides nothing. */
+size_t yd_shard_wait_for_starting_task_rpcs(yd_sched* s, int64_t now_ns, const yd_rpc_wait* rpcs, size_t n_rpcs,
+                                            yd_rpc_wait_result* results, yd_grant* grants_out, size_t cap);
+/* A SchedulerServiceImpl over the group (ydservice.h; ydwire.h works on it unchanged).  Collective; every rank passes the
+ * same config.  Its handlers make the replicated calls above: Heartbeat's notification, WaitForStartingTask,
+ * KeepTaskAlive, GetRunningTasks, and FreeTask through yd_shard_free_tasks (rank 0 passes the ids).  KeepServantAlive is
+ * the per-rank call, fed to every rank alike.  The serving-daemon tokens are rank 0's, through one all-gather at
+ * creation and one per roll-out.  Fed the same calls, every rank's service returns the same answers (and the wire
+ * layer writes the same bytes).  Returns NULL on every rank if the handle has not joined a group or the config is
+ * refused (as yd_service_create). */
+yd_service* yd_shard_service_create(yd_sched* s, int64_t now_ns, const yd_service_config* cfg);
 
 /* Device time (ms, CUDA events on the solve stream) of the last sharded solve's phases: local kernels and
  * the four exchanges.  Returns 0 if there was none. */

@@ -311,6 +311,13 @@ SHARD_PROTOTYPES = [
     ("yd_shard_last_stats", C.c_int, [_P, C.POINTER(yd_shard_stats)]),
     ("yd_shard_export_state", C.c_size_t, [_P, C.c_int64, _P, C.c_size_t]),
     ("yd_shard_import_state", C.c_int, [_P, C.c_int64, _P, C.c_size_t]),
+    ("yd_shard_keep_task_alive", C.c_int, [_P, C.c_int64, _P, C.c_size_t, C.c_int64, _P]),
+    ("yd_shard_notify_servants_running_tasks", C.c_size_t,
+     [_P, C.POINTER(yd_heartbeat_item), C.c_size_t, C.POINTER(C.c_uint64), C.POINTER(C.c_size_t)]),
+    ("yd_shard_get_running_tasks", C.c_size_t, [_P, C.POINTER(yd_running_task), C.c_size_t]),
+    ("yd_shard_running_index_refresh", C.c_size_t, [_P]),
+    ("yd_shard_wait_for_starting_task_rpcs", C.c_size_t, [_P, C.c_int64, _P, C.c_size_t, _P, _P, C.c_size_t]),
+    ("yd_shard_service_create", _P, [_P, C.c_int64, C.POINTER(yd_service_config)]),
 ]
 
 # Every symbol include/ydstate.h declares, and its status codes.

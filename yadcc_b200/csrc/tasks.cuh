@@ -298,8 +298,10 @@ __global__ void k_free(const unsigned long long* __restrict__ ids, uint32_t n, T
 }
 
 // ---- KeepTaskAlive (cc:142-165) ----------------------------------------------
+// `ok` is bytes for one handle, u32 words for a range-sharded group (the words travel in a sum all-reduce).
+template <typename Flag>
 __global__ void k_keep_alive(const unsigned long long* __restrict__ ids, uint32_t n, long long now_ns,
-                             long long new_expires_in_ns, TaskRing ring, uint8_t* __restrict__ ok) {
+                             long long new_expires_in_ns, TaskRing ring, Flag* __restrict__ ok) {
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   unsigned long long id;
@@ -446,8 +448,11 @@ __global__ void k_notify_sweep(TaskRing ring, NotifyBatch b, uint32_t* __restric
 }
 
 // Check: a reported id is "permitted" iff it is a live, non-zombie grant on the reporting
-// servant (cc:257-262); everything else goes back to the daemon as unknown.  One thread per id.
-__global__ void k_notify_check(TaskRing ring, NotifyBatch b, uint32_t n_ids, uint8_t* __restrict__ permitted) {
+// servant (cc:257-262); everything else goes back to the daemon as unknown.  One thread per id.  A permitted id gets
+// `tag`: 1 in bytes for one handle; rank + 1 in u32 words for a range-sharded group, whose sum over the ranks then says
+// both whether and where the lease lives (it lives on one rank at most).
+template <typename Flag>
+__global__ void k_notify_check(TaskRing ring, NotifyBatch b, uint32_t n_ids, Flag* __restrict__ permitted, Flag tag) {
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_ids) return;
   uint32_t lo = 0, hi = b.n_items;  // the item whose id range holds i
@@ -463,7 +468,7 @@ __global__ void k_notify_check(TaskRing ring, NotifyBatch b, uint32_t n_ids, uin
     uint32_t f = ring.flags[slot];
     ok = (f & kTaskAlive) && !(f & kTaskZombie) && ring.srv[slot] == pos;
   }
-  permitted[i] = ok;
+  permitted[i] = ok ? tag : Flag(0);
 }
 
 // Ring growth: re-place the live window into a ring twice (or more) the size.

@@ -1906,14 +1906,21 @@ namespace {
 // NotifyServantRunningTasks (cc:222-277) for heartbeats of DISTINCT known servants: one upload, one
 // sweep + one check kernel, one synchronisation, whatever the number of servants or reported tasks.
 // `idx` = the items of the caller's array handled here, `pos` their registry positions.
+// A range-sharded group's call (d_flags != nullptr) leaves the verdicts on the device instead: `tag` (rank + 1) per
+// permitted id, as u32 words at d_flags[item_at[i] ..] for item i, the pass's items in registry order from `base`.  It neither
+// downloads nor synchronises: the caller does, once, after the exchange.
 void NotifyDistinct(yd_sched* s, const yd_heartbeat_item* items, const std::vector<uint32_t>& idx,
-                    const std::vector<uint32_t>& pos, std::vector<std::vector<uint8_t>>& permitted) {
+                    const std::vector<uint32_t>& pos, std::vector<std::vector<uint8_t>>& permitted,
+                    uint32_t* d_flags = nullptr, uint32_t tag = 0, size_t base = 0, std::vector<size_t>* item_at = nullptr) {
   const uint32_t m = (uint32_t)idx.size();
   std::vector<uint32_t> order(m);
   std::iota(order.begin(), order.end(), 0u);
   std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return pos[a] < pos[b]; });
   size_t total = 0;
-  for (uint32_t k = 0; k != m; ++k) total += items[idx[k]].n_tasks;
+  for (uint32_t k = 0; k != m; ++k) {
+    if (item_at) (*item_at)[idx[order[k]]] = base + total;
+    total += items[idx[order[k]]].n_tasks;
+  }
   if (total > 0xfffffff0ull) { fprintf(stderr, "ydsched: heartbeat batch reports too many tasks\n"); abort(); }
   const bool window = s->next_id > s->lo;
   if (!window || (total == 0 && s->zombies_ub == 0)) return;  // nothing can be permitted, nothing to sweep
@@ -1949,8 +1956,16 @@ void NotifyDistinct(yd_sched* s, const yd_heartbeat_item* items, const std::vect
                                                                        s->shard ? s->d_dec.as<uint32_t>() : nullptr);
     YD_CUDA_CHECK(cudaGetLastError());
   }
+  if (d_flags) {
+    if (total) {
+      yd::k_notify_check<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(s->ring(), nb, (uint32_t)total, d_flags + base, tag);
+      YD_CUDA_CHECK(cudaGetLastError());
+    }
+    return;
+  }
   if (total) {
-    yd::k_notify_check<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(s->ring(), nb, (uint32_t)total, s->d_ok.as<uint8_t>());
+    yd::k_notify_check<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(s->ring(), nb, (uint32_t)total, s->d_ok.as<uint8_t>(),
+                                                                        uint8_t(1));
     YD_CUDA_CHECK(cudaGetLastError());
     YD_CUDA_CHECK(cudaMemcpyAsync(h_ok, s->d_ok.p, total, cudaMemcpyDeviceToHost, st));
   }
@@ -1961,34 +1976,36 @@ void NotifyDistinct(yd_sched* s, const yd_heartbeat_item* items, const std::vect
     if (total) memcpy(p.data(), h_ok + h_off[k], p.size());
   }
 }
-}  // namespace
-}  // extern "C++"
 
-// NotifyServantRunningTasks x n, in array order (cc:222-277).
-size_t yd_notify_servants_running_tasks(yd_sched* s, const yd_heartbeat_item* items, size_t n, uint64_t* unknown_out,
-                                        size_t* unknown_counts) {
-  YD_CUDA_CHECK(cudaSetDevice(s->device));
-  s->SyncServantState();
-  std::vector<std::vector<uint8_t>> permitted(n);
-  for (size_t i = 0; i != n; ++i) permitted[i].assign(items[i].n_tasks, 0);
-  // Heartbeats of different servants touch disjoint leases, so any number of them is one device pass.
-  // A servant that appears twice must see its first heartbeat's sweep: the batch is cut there.
+// The items' registry positions (kNone: the servant itself expired, every id is unknown, cc:243-245) and the passes
+// of NotifyDistinct, `pass(idx, pos)` each.  Heartbeats of different servants touch disjoint leases, so any number of
+// them is one device pass.  A servant that appears twice must see its first heartbeat's sweep: the batch is cut there.
+template <typename Pass>
+std::vector<uint32_t> NotifyPasses(yd_sched* s, const yd_heartbeat_item* items, size_t n, Pass&& pass) {
   std::vector<uint32_t> idx, pos;
   std::unordered_map<uint32_t, char> seen;
   std::vector<uint32_t> item_pos(n, kNone);
   for (size_t i = 0; i != n; ++i) {
     auto it = s->loc2pos.find(items[i].servant_location ? items[i].servant_location : "");
-    if (it == s->loc2pos.end()) continue;  // the servant itself expired: every id is unknown (cc:243-245)
+    if (it == s->loc2pos.end()) continue;
     item_pos[i] = it->second;
     if (seen.count(it->second)) {
-      NotifyDistinct(s, items, idx, pos, permitted);
+      pass(idx, pos);
       idx.clear(); pos.clear(); seen.clear();
     }
     seen.emplace(it->second, 1);
     idx.push_back((uint32_t)i);
     pos.push_back(it->second);
   }
-  if (!idx.empty()) NotifyDistinct(s, items, idx, pos, permitted);
+  if (!idx.empty()) pass(idx, pos);
+  return item_pos;
+}
+
+// The answer, in request order, and the bookkeeper's update.  verdict(i, t) of task t of item i: 0 unknown, 1 permitted
+// and kept here, 2 permitted and kept by the rank of a range-sharded group that holds its lease.
+template <typename Verdict>
+size_t NotifyAnswer(yd_sched* s, const yd_heartbeat_item* items, size_t n, const std::vector<uint32_t>& item_pos,
+                    Verdict&& verdict, uint64_t* unknown_out, size_t* unknown_counts) {
   size_t total = 0;
   for (size_t i = 0; i != n; ++i) {
     const yd_heartbeat_item& it = items[i];
@@ -1998,9 +2015,10 @@ size_t yd_notify_servants_running_tasks(yd_sched* s, const yd_heartbeat_item* it
     } else {
       std::vector<RunningRec> kept;
       for (size_t t = 0; t != it.n_tasks; ++t) {
-        if (!permitted[i][t]) {
+        const int v = verdict(i, t);
+        if (v == 0) {
           unknown_out[total + k++] = it.tasks[t].task_grant_id;
-        } else {
+        } else if (v == 1) {
           kept.push_back(RunningRec{it.tasks[t].servant_task_id, it.tasks[t].task_grant_id,
                                     it.tasks[t].servant_location ? it.tasks[t].servant_location : "",
                                     it.tasks[t].task_digest ? it.tasks[t].task_digest : "", (uint32_t)t});
@@ -2014,6 +2032,21 @@ size_t yd_notify_servants_running_tasks(yd_sched* s, const yd_heartbeat_item* it
     total += k;
   }
   return total;
+}
+}  // namespace
+}  // extern "C++"
+
+// NotifyServantRunningTasks x n, in array order (cc:222-277).
+size_t yd_notify_servants_running_tasks(yd_sched* s, const yd_heartbeat_item* items, size_t n, uint64_t* unknown_out,
+                                        size_t* unknown_counts) {
+  YD_CUDA_CHECK(cudaSetDevice(s->device));
+  s->SyncServantState();
+  std::vector<std::vector<uint8_t>> permitted(n);
+  for (size_t i = 0; i != n; ++i) permitted[i].assign(items[i].n_tasks, 0);
+  const std::vector<uint32_t> item_pos = NotifyPasses(
+      s, items, n, [&](const std::vector<uint32_t>& idx, const std::vector<uint32_t>& pos) { NotifyDistinct(s, items, idx, pos, permitted); });
+  return NotifyAnswer(
+      s, items, n, item_pos, [&](size_t i, size_t t) { return permitted[i][t] ? 1 : 0; }, unknown_out, unknown_counts);
 }
 
 // NotifyServantRunningTasks, cc:222-277: a batch of one.
@@ -2208,18 +2241,8 @@ static yd::RtIndex MakeRtIndex(yd_sched* s) {
   return ix;
 }
 
-// RunningTaskKeeper::Refresh, running_task_keeper.cc:40-65.
-size_t yd_running_index_refresh(yd_sched* s) {
-  // the snapshot: what GetRunningTasks answers now (running_task_bookkeeper.cc:36-43)
-  // (each servant's list goes to the FRONT there: same order, built back to front in O(n))
-  s->rt_snapshot.clear();
-  {
-    std::vector<const std::vector<RunningRec>*> groups;
-    for (auto&& [k, v] : s->running) groups.push_back(&v);
-    for (auto it = groups.rbegin(); it != groups.rend(); ++it) {
-      s->rt_snapshot.insert(s->rt_snapshot.end(), (*it)->begin(), (*it)->end());
-    }
-  }
+// The index over s->rt_snapshot (running_index.cuh).  Returns the number of entries.
+static size_t RtIndexBuild(yd_sched* s) {
   const size_t n = s->rt_snapshot.size();
   s->rt_distinct = 0;
   if (n == 0) return 0;
@@ -2260,6 +2283,21 @@ size_t yd_running_index_refresh(yd_sched* s) {
   YD_CUDA_CHECK(cudaStreamSynchronize(st));  // also keeps the pageable staging vectors alive long enough
   s->rt_distinct = h_distinct;
   return n;
+}
+
+// RunningTaskKeeper::Refresh, running_task_keeper.cc:40-65.
+size_t yd_running_index_refresh(yd_sched* s) {
+  // the snapshot: what GetRunningTasks answers now (running_task_bookkeeper.cc:36-43)
+  // (each servant's list goes to the FRONT there: same order, built back to front in O(n))
+  s->rt_snapshot.clear();
+  {
+    std::vector<const std::vector<RunningRec>*> groups;
+    for (auto&& [k, v] : s->running) groups.push_back(&v);
+    for (auto it = groups.rbegin(); it != groups.rend(); ++it) {
+      s->rt_snapshot.insert(s->rt_snapshot.end(), (*it)->begin(), (*it)->end());
+    }
+  }
+  return RtIndexBuild(s);
 }
 
 size_t yd_running_index_size(yd_sched* s) { return s->rt_distinct; }
@@ -2953,3 +2991,5 @@ extern "C" int yd_shard_import_state(yd_sched* s, int64_t now_ns, const uint8_t*
   ApplyImport(s, now_ns, im, R, W);
   return YD_STATE_OK;
 }
+
+#include "shard_calls.inc"

@@ -334,13 +334,15 @@ class TaskDispatcher:
         """A batch of SchedulerServiceImpl::WaitForStartingTask bodies
         (scheduler_service_impl.cc:209-271): returns (results, grants) where
         results[i] = (status, n_grants, first_grant) and grants is a GRANT_DTYPE array."""
+        return self._rpcs_with(self._lib.yd_wait_for_starting_task_rpcs, rpcs, now)
+
+    def _rpcs_with(self, fn, rpcs: np.ndarray, now: float):
         assert rpcs.dtype == _abi.RPC_WAIT_DTYPE and rpcs.flags.c_contiguous
         n = rpcs.shape[0]
         cap = int(self._lib.yd_rpc_expanded_requests(self._h, rpcs.ctypes.data, n))  # counts clamped to what can be granted
         results = np.zeros(n, dtype=_abi.RPC_RESULT_DTYPE)
         grants = np.zeros(max(cap, 1), dtype=GRANT_DTYPE)
-        k = self._lib.yd_wait_for_starting_task_rpcs(self._h, _ns(now), rpcs.ctypes.data, n, results.ctypes.data,
-                                                     grants.ctypes.data, cap)
+        k = fn(self._h, _ns(now), rpcs.ctypes.data, n, results.ctypes.data, grants.ctypes.data, cap)
         if k == (1 << 64) - 1:
             raise ValueError("grant buffer too small")
         return results, grants[:k]
@@ -349,9 +351,13 @@ class TaskDispatcher:
         return bool(self.keep_tasks_alive([task_id], new_expires_in, now=now)[0])
 
     def keep_tasks_alive(self, task_ids: Iterable[int], new_expires_in: float, *, now: float = 0.0) -> np.ndarray:
+        return self._keep_alive_with(self._lib.yd_keep_task_alive, task_ids, new_expires_in, now)
+
+    def _keep_alive_with(self, fn, task_ids, new_expires_in: float, now: float) -> np.ndarray:
         ids = np.ascontiguousarray(np.asarray(list(task_ids) if not isinstance(task_ids, np.ndarray) else task_ids, dtype=np.uint64))
         ok = np.zeros(ids.shape[0], dtype=np.uint8)
-        self._lib.yd_keep_task_alive(self._h, _ns(now), ids.ctypes.data, ids.shape[0], _ns(new_expires_in), ok.ctypes.data)
+        if fn(self._h, _ns(now), ids.ctypes.data, ids.shape[0], _ns(new_expires_in), ok.ctypes.data):
+            raise RuntimeError("keep-alive refused")
         return ok.astype(bool)
 
     def free_task(self, task_id: int) -> None:
@@ -400,6 +406,9 @@ class TaskDispatcher:
 
     def notify_servants_running_tasks(self, batch: Sequence[tuple[str, Sequence[RunningTask]]]) -> list[list[int]]:
         """NotifyServantRunningTasks for many servants in one call: [(location, tasks)] -> unknown ids per item."""
+        return self._notify_with(self._lib.yd_notify_servants_running_tasks, batch)
+
+    def _notify_with(self, fn, batch) -> list[list[int]]:
         n = len(batch)
         items = (_abi.yd_heartbeat_item * max(n, 1))()
         keep = []
@@ -417,7 +426,7 @@ class TaskDispatcher:
             total += m
         out = (C.c_uint64 * max(total, 1))()
         counts = (C.c_size_t * max(n, 1))()
-        self._lib.yd_notify_servants_running_tasks(self._h, items, n, out, counts)
+        fn(self._h, items, n, out, counts)
         res, at = [], 0
         for i in range(n):
             res.append([int(out[at + k]) for k in range(counts[i])])
@@ -437,9 +446,12 @@ class TaskDispatcher:
         return [int(out[i]) for i in range(k)]
 
     def get_running_tasks(self) -> list[RunningTask]:
-        n = self._lib.yd_get_running_tasks(self._h, None, 0)
+        return self._running_with(self._lib.yd_get_running_tasks)
+
+    def _running_with(self, fn) -> list[RunningTask]:
+        n = fn(self._h, None, 0)
         arr = (_abi.yd_running_task * max(n, 1))()
-        n = min(n, self._lib.yd_get_running_tasks(self._h, arr, n))
+        n = min(n, fn(self._h, arr, n))
         return [
             RunningTask(
                 int(arr[i].servant_task_id),

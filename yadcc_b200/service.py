@@ -54,11 +54,30 @@ class SchedulerService:
     def __init__(self, dispatcher: TaskDispatcher, *, acceptable_user_tokens: str, acceptable_servant_tokens: str,
                  min_daemon_version: int = 0, serving_daemon_token_rollout_interval: int = 3600, token_seed: int = 0,
                  now: float = 0.0):
+        """`dispatcher` may also be a RangeShardedDispatcher: the service then answers for the whole group
+        (yd_shard_service_create).  Building it is collective, and every rank's service must be fed the same calls;
+        every rank then gives the same answers and hands out rank 0's serving-daemon tokens."""
+        group = None
+        if not isinstance(dispatcher, TaskDispatcher):  # a RangeShardedDispatcher
+            group, dispatcher = dispatcher, dispatcher.local
+        self.group = group
         self.dispatcher = dispatcher
         self._lib = dispatcher._lib
+        create = self._lib.yd_service_create
+        if group is not None and group.native:
+            create = self._lib.yd_shard_service_create
+        elif group is not None and token_seed == 0 and group.world > 1:
+            # replicas over gloo: the same tokens on every rank from a seed rank 0 draws
+            import secrets
+
+            import torch.distributed as dist
+
+            seeds: list = [None] * group.world
+            dist.all_gather_object(seeds, secrets.randbits(64) or 1, group=group.group)
+            token_seed = seeds[0]
         cfg = _abi.yd_service_config(acceptable_user_tokens.encode(), acceptable_servant_tokens.encode(),
                                      min_daemon_version, serving_daemon_token_rollout_interval, token_seed)
-        self._h = self._lib.yd_service_create(dispatcher._h, _ns(now), C.byref(cfg))
+        self._h = create(dispatcher._h, _ns(now), C.byref(cfg))
         if not self._h:
             raise ValueError("both token lists must be non-empty (token_verifier.cc:58-59)")
 

@@ -283,6 +283,39 @@ class RangeShardedDispatcher:
         if rc != 0:
             raise RuntimeError(f"yd_shard_free_tasks failed: {rc}")
 
+    # -- replicated calls (ydshard.h): every rank makes the call with the same arguments and gets the single scheduler's
+    # answer.  Over gloo with the CPU libraries every replica holds every lease, so these are the local calls there.
+    def keep_tasks_alive(self, ids, new_expires_in: float, *, now: float = 0.0) -> np.ndarray:
+        """Replicated KeepTaskAlive: the holder of each lease renews it; every rank returns the same flags."""
+        if not self.native:
+            return self.local.keep_tasks_alive(ids, new_expires_in, now=now)
+        return self.local._keep_alive_with(self.local._lib.yd_shard_keep_task_alive, ids, new_expires_in, now)
+
+    def notify_servants_running_tasks(self, batch) -> list[list[int]]:
+        """Replicated NotifyServantRunningTasks for [(location, tasks)]: an id is unknown iff no rank holds its lease."""
+        if not self.native:
+            return self.local.notify_servants_running_tasks(batch)
+        return self.local._notify_with(self.local._lib.yd_shard_notify_servants_running_tasks, batch)
+
+    def get_running_tasks(self):
+        """Replicated GetRunningTasks: the whole group's list, in the single scheduler's order."""
+        if not self.native:
+            return self.local.get_running_tasks()
+        return self.local._running_with(self.local._lib.yd_shard_get_running_tasks)
+
+    def running_index_refresh(self) -> int:
+        """Replicated RunningTaskKeeper::Refresh: afterwards `local.find_running_tasks` answers for the whole group."""
+        if not self.native:
+            return self.local.running_index_refresh()
+        return int(self.local._lib.yd_shard_running_index_refresh(self.local._h))
+
+    def wait_for_starting_task_rpcs(self, rpcs: np.ndarray, now: float = 0.0):
+        """Replicated window of WaitForStartingTask RPCs: every rank passes the whole window and gets (results, grants)
+        for all of it; each rank decides an even share of the expanded queue."""
+        if not self.native:
+            return self.local.wait_for_starting_task_rpcs(rpcs, now)
+        return self.local._rpcs_with(self.local._lib.yd_shard_wait_for_starting_task_rpcs, rpcs, now)
+
     def export_state(self, now: float = 0.0) -> bytes:
         """Collective.  The group's state as ONE scheduler's export (ydstate.h), the same bytes on every rank: a
         single TaskDispatcher, or a group of any size, can import it (import_state)."""

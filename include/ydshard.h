@@ -27,6 +27,7 @@
 #ifndef YDSHARD_H_
 #define YDSHARD_H_
 
+#include "ydkeys.h"
 #include "ydsched.h"
 #include "ydservice.h"
 
@@ -124,6 +125,46 @@ size_t yd_shard_wait_for_starting_task_rpcs(yd_sched* s, int64_t now_ns, const y
  * layer writes the same bytes).  Returns NULL on every rank if the handle has not joined a group or the config is
  * refused (as yd_service_create). */
 yd_service* yd_shard_service_create(yd_sched* s, int64_t now_ns, const yd_service_config* cfg);
+
+/* THE PRE-FILTERED SOLVE OVER A GROUP (BASELINE configs[3]; yd_filter_and_wait_for_starting_new_tasks, ydsched.h, and
+ * yd_derive_filter_and_wait_for_starting_new_tasks, ydkeys.h).  Collective: the whole queue is the ranks' `reqs_local`
+ * concatenated in rank order, as in yd_shard_wait_for_starting_new_tasks.  Each rank runs the filter stages (the key
+ * derivation, the bloom probe, the in-flight index probe and the order-keeping compaction) on its own range on its own
+ * GPU, then every rank enters the sharded solve with its offered requests, also a rank whose range is empty or filtered
+ * out entirely.  The answers equal those of one handle given the concatenated queue through the single-handle call:
+ * verdict_out[i] and hits_out[i] (may be NULL) belong to the i-th request of this rank's range; grants_out[0 .. returned)
+ * are the grants of this rank's OFFERED requests, in order; task ids number the grants of the group's whole offered queue
+ * in FIFO order; afterwards every replica's running_tasks and next task id are the single handle's.  Returns how many of
+ * this rank's requests were offered.
+ *
+ * Not checked across ranks, as in the other replicated calls: the bloom filters (each rank probes its own, so the ranks
+ * hold the same one: yd_bloom_reset / yd_bloom_load / yd_bloom_add fed alike) and the in-flight index (hits_out[i].
+ * snapshot_index refers to the group snapshot when it was last refreshed with yd_shard_running_index_refresh on every
+ * rank).  Programmer errors abort as in the single-handle calls (a bloom filter used before yd_bloom_reset / _load, keys
+ * longer than the bloom filter takes, more than 2^30 requests).
+ *
+ * Afterwards each rank's staging area holds exactly its offered requests, in order (none if it offered none), so
+ * yd_shard_wait_for_starting_new_tasks(s, now, NULL, offered, out) decides them again.  A refusal returns (size_t)-1 on
+ * every rank and decides nothing: capacities above 8192 per servant (replicated state: every rank sees it before any
+ * stage, and the staged queues are kept), or the sharded solve's own refusals (then after the stages: the staging areas
+ * hold the offered requests).  On a handle that has not joined a group, these are the single-handle calls.
+ *
+ * yd_last_solve_stats then reports the rank's stages: prep_ms (= total_ms) is their device time (derivation, filter
+ * stages, compaction), decisions = n_local, granted = this rank's grants; yd_shard_last_stats describes the solve. */
+size_t yd_shard_filter_and_wait_for_starting_new_tasks(yd_sched* s, int64_t now_ns, const yd_task_req* reqs_local,
+                                                       size_t n_local, const yd_prefilter* filter, uint8_t* verdict_out,
+                                                       yd_running_hit* hits_out, yd_grant* grants_out);
+/* The same from task descriptors: each rank's `src_local` describes its own range with its own argument table, and the
+ * equivalent single-handle queue appends the ranks' argument tables in rank order, each rank's args_index shifted by the
+ * earlier ranks' n_args (the ranks pass the same source_digest_len, which is not checked).  `stages` is YD_STAGE_* and
+ * must be the same on every rank.  If any rank's descriptors are refused (a YD_KEYS_* code of yd_derive_task_keys), every
+ * rank returns (size_t)-1, decides nothing and keeps its staged queue: the ranks agree on this through one small
+ * all-gather before anything is uploaded.  The keys each request needs depend on that request alone, so the derivation,
+ * the call's most expensive stage, is split over the GPUs with the ranges. */
+size_t yd_shard_derive_filter_and_wait_for_starting_new_tasks(yd_sched* s, int64_t now_ns, const yd_task_req* reqs_local,
+                                                              size_t n_local, const yd_task_sources* src_local,
+                                                              uint32_t stages, uint8_t* verdict_out,
+                                                              yd_running_hit* hits_out, yd_grant* grants_out);
 
 /* Device time (ms, CUDA events on the solve stream) of the last sharded solve's phases: local kernels and
  * the four exchanges.  Returns 0 if there was none. */

@@ -318,6 +318,9 @@ SHARD_PROTOTYPES = [
     ("yd_shard_running_index_refresh", C.c_size_t, [_P]),
     ("yd_shard_wait_for_starting_task_rpcs", C.c_size_t, [_P, C.c_int64, _P, C.c_size_t, _P, _P, C.c_size_t]),
     ("yd_shard_service_create", _P, [_P, C.c_int64, C.POINTER(yd_service_config)]),
+    ("yd_shard_filter_and_wait_for_starting_new_tasks", C.c_size_t, [_P, C.c_int64, _P, C.c_size_t, _P, _P, _P, _P]),
+    ("yd_shard_derive_filter_and_wait_for_starting_new_tasks", C.c_size_t,
+     [_P, C.c_int64, _P, C.c_size_t, _P, C.c_uint32, _P, _P, _P]),
 ]
 
 # Every symbol include/ydstate.h declares, and its status codes.

@@ -41,6 +41,7 @@
 #include "state.cuh"
 #include "ydstate_codec.inc"
 #include "ydkeys.h"
+#include "ydshard.h"
 #include "ydsched_keys_impl.inc"
 
 namespace {
@@ -2348,11 +2349,36 @@ static void FilterPrepare(yd_sched* s, uint32_t N, bool bloom, size_t key_span, 
   }
 }
 
+// The last step of the pre-filtered solve on a rank of a range-sharded group: the sharded solve of the `kept` requests
+// the compaction staged (of N).  Every rank enters it, also one that kept nothing.  Leaves the stats of the solve reset
+// (the solve is yd_shard_last_stats'), with decisions = N and this rank's grants.  Returns kept, or (size_t)-1 if the
+// sharded solve refused the batch (on every rank: its refusals depend on replicated state only).
+static size_t ShardSolveKept(yd_sched* s, int64_t now_ns, uint32_t N, uint32_t kept, yd_grant* grants_out) {
+  s->staged_n = kept;
+  const int rc = yd_shard_wait_for_starting_new_tasks(s, now_ns, nullptr, kept, grants_out);
+  if (kept && s->staged_n != kept) {
+    // decided through the gathered queue, which went through the staging area: compact the offered requests there again
+    yd::k_keep_scatter<<<(N + 1023) / 1024, 1024, 0, s->st>>>(s->d_freqs.as<yd_task_req>(), s->d_fverdict.as<uint8_t>(),
+                                                              s->d_ftile.as<uint32_t>(), N, s->d_reqs.as<yd_task_req>());
+    YD_CUDA_CHECK(cudaGetLastError());
+    YD_CUDA_CHECK(cudaStreamSynchronize(s->st));
+    s->staged_n = kept;
+  }
+  s->stats = yd_solve_stats{};
+  s->stats_times_pending = 0;
+  s->have_stats = true;
+  s->stats.decisions = N;
+  if (rc) return (size_t)-1;
+  for (uint32_t i = 0; i != kept; ++i) s->stats.granted += grants_out[i].status == YD_STATUS_GRANTED;
+  return kept;
+}
+
 // The device part of the pre-filtered solve, from the first filter stage on: the queue is in d_freqs, the cache keys
-// (if `bloom`) in d_bloom_keys, the task digests (if `dedupe`) in d_rt_keys, and ev_f[0] has been recorded.
+// (if `bloom`) in d_bloom_keys, the task digests (if `dedupe`) in d_rt_keys, and ev_f[0] has been recorded.  The solve of
+// the compacted queue is the single handle's, or with `group` the range-sharded group's.
 static size_t FilterStages(yd_sched* s, int64_t now_ns, uint32_t N, bool bloom, size_t key_len, size_t key_stride, bool dedupe,
                            size_t digest_len, size_t digest_stride, uint8_t* verdict_out, yd_running_hit* hits_out,
-                           yd_grant* grants_out, size_t h2d_bytes, uint32_t extra_launches) {
+                           yd_grant* grants_out, size_t h2d_bytes, uint32_t extra_launches, bool group) {
   cudaStream_t st = s->st;
   const size_t n = N;
   const uint32_t nt = (N + 1023) / 1024;
@@ -2383,7 +2409,11 @@ static size_t FilterStages(yd_sched* s, int64_t now_ns, uint32_t N, bool bloom, 
   const uint32_t kept = *s->h_fcount.as<uint32_t>();
   float filter_ms = 0;
   cudaEventElapsedTime(&filter_ms, s->ev_f[0], s->ev_f[1]);
-  if (kept) {
+  size_t ret = kept;
+  if (group) {
+    ret = ShardSolveKept(s, now_ns, N, kept, grants_out);
+    s->stats.total_ms = filter_ms;
+  } else if (kept) {
     s->staged_n = kept;  // the compaction wrote the solver's queue
     WaitImpl(s, now_ns, nullptr, nullptr, kept, grants_out, nullptr, nullptr);
     yd_solve_stats st2;
@@ -2399,15 +2429,15 @@ static size_t FilterStages(yd_sched* s, int64_t now_ns, uint32_t N, bool bloom, 
   s->stats.kernel_launches += 3 + (bloom ? 1 : 0) + (dedupe ? 1 : 0) + extra_launches;
   s->stats.h2d_bytes += h2d_bytes;
   s->stats.d2h_bytes += N + 4 + (hits_out && dedupe ? n * sizeof(yd_running_hit) : 0);
-  return kept;
+  return ret;
 }
 
 // BASELINE configs[3] in one call: bloom probes, in-flight index probes, order-preserving compaction and the solve,
-// with the queue resident in HBM from the first stage to the last (filter.cuh).
-size_t yd_filter_and_wait_for_starting_new_tasks(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, size_t n,
-                                                 const yd_prefilter* f, uint8_t* verdict_out, yd_running_hit* hits_out,
-                                                 yd_grant* grants_out) {
-  if (n == 0) return 0;
+// with the queue resident in HBM from the first stage to the last (filter.cuh).  `group`: the solve is the range-sharded
+// group's (yd_shard_filter_and_wait_for_starting_new_tasks).
+static size_t FilterCall(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, size_t n, const yd_prefilter* f,
+                         uint8_t* verdict_out, yd_running_hit* hits_out, yd_grant* grants_out, bool group) {
+  if (n == 0) return group ? ShardSolveKept(s, now_ns, 0, 0, grants_out) : 0;
   if (n > 0x40000000ull) { fprintf(stderr, "ydsched: batch too large\n"); abort(); }
   YD_CUDA_CHECK(cudaSetDevice(s->device));
   cudaStream_t st = s->st;
@@ -2427,7 +2457,13 @@ size_t yd_filter_and_wait_for_starting_new_tasks(yd_sched* s, int64_t now_ns, co
   YD_CUDA_CHECK(cudaEventRecord(s->ev_f[0], st));
   return FilterStages(s, now_ns, N, bloom, bloom ? f->cache_key_len : 0, bloom ? f->cache_key_stride : 0, dedupe,
                       dedupe ? f->task_digest_len : 0, dedupe ? f->task_digest_stride : 0, verdict_out, hits_out, grants_out,
-                      size_t(N) * sizeof(yd_task_req) + key_span + digest_span, 0);
+                      size_t(N) * sizeof(yd_task_req) + key_span + digest_span, 0, group);
+}
+
+size_t yd_filter_and_wait_for_starting_new_tasks(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, size_t n,
+                                                 const yd_prefilter* f, uint8_t* verdict_out, yd_running_hit* hits_out,
+                                                 yd_grant* grants_out) {
+  return FilterCall(s, now_ns, reqs, n, f, verdict_out, hits_out, grants_out, false);
 }
 
 // ---- cache keys and task digests from task descriptors (blake3.cuh) ------------------------------------------------
@@ -2540,12 +2576,12 @@ int yd_derive_task_keys(yd_sched* s, const yd_task_req* reqs, size_t n, const yd
 }
 
 // The pre-filtered solve from descriptors: the keys are derived straight into d_bloom_keys / d_rt_keys, at the strides
-// the filter stages read, so from there on it is yd_filter_and_wait_for_starting_new_tasks' device part unchanged.
-size_t yd_derive_filter_and_wait_for_starting_new_tasks(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, size_t n,
-                                                        const yd_task_sources* src, uint32_t stages, uint8_t* verdict_out,
-                                                        yd_running_hit* hits_out, yd_grant* grants_out) {
-  if (yd_keys_check(s->envs, reqs, n, src) != YD_KEYS_OK) return (size_t)-1;
-  if (n == 0) return 0;
+// the filter stages read, so from there on it is yd_filter_and_wait_for_starting_new_tasks' device part unchanged.  The
+// descriptors have passed yd_keys_check.  `group`: the solve is the range-sharded group's.
+static size_t DeriveFilterCall(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, size_t n, const yd_task_sources* src,
+                               uint32_t stages, uint8_t* verdict_out, yd_running_hit* hits_out, yd_grant* grants_out,
+                               bool group) {
+  if (n == 0) return group ? ShardSolveKept(s, now_ns, 0, 0, grants_out) : 0;
   if (n > 0x40000000ull) { fprintf(stderr, "ydsched: batch too large\n"); abort(); }
   const bool bloom = stages & YD_STAGE_CACHE, dedupe = stages & YD_STAGE_DEDUPE;
   if (bloom && !s->bloom_bits) { fprintf(stderr, "ydsched: bloom filter used before yd_bloom_reset / yd_bloom_load\n"); abort(); }
@@ -2567,7 +2603,14 @@ size_t yd_derive_filter_and_wait_for_starting_new_tasks(yd_sched* s, int64_t now
   }
   return FilterStages(s, now_ns, N, bloom, YD_KEYS_CACHE_KEY_LEN, YD_KEYS_CACHE_KEY_LEN, dedupe, YD_KEYS_TASK_DIGEST_LEN,
                       YD_KEYS_TASK_DIGEST_LEN, verdict_out, hits_out, grants_out, size_t(N) * sizeof(yd_task_req) + k.h2d,
-                      (bloom || dedupe) ? 1u : 0u);
+                      (bloom || dedupe) ? 1u : 0u, group);
+}
+
+size_t yd_derive_filter_and_wait_for_starting_new_tasks(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, size_t n,
+                                                        const yd_task_sources* src, uint32_t stages, uint8_t* verdict_out,
+                                                        yd_running_hit* hits_out, yd_grant* grants_out) {
+  if (yd_keys_check(s->envs, reqs, n, src) != YD_KEYS_OK) return (size_t)-1;
+  return DeriveFilterCall(s, now_ns, reqs, n, src, stages, verdict_out, hits_out, grants_out, false);
 }
 
 

@@ -114,6 +114,27 @@ class TaskSources:
         blob = np.frombuffer(b"".join(b) or b"\0", dtype=np.uint8).copy()
         return cls(blob, off, np.ascontiguousarray(args_index, dtype=np.uint32), TaskDispatcher._key_matrix(source_digests))
 
+    @classmethod
+    def concat(cls, parts: Sequence["TaskSources"], counts: Sequence[int]) -> "TaskSources":
+        """The descriptors of several queues, concatenated: parts[r] describes counts[r] requests.  The argument tables
+        are appended in order and each part's args_index is shifted by the earlier parts' string counts (the queue a
+        range-sharded group's ranks describe together, include/ydshard.h)."""
+        blobs, offs, idx, sds = [], [np.zeros(1, dtype=np.uint64)], [], []
+        nbytes = nargs = 0
+        for p, n in zip(parts, counts):
+            end = int(p.args_offsets[-1])
+            blobs.append(p.args[:end])
+            offs.append(p.args_offsets[1:] + np.uint64(nbytes))
+            idx.append(p.args_index[:n].astype(np.uint32) + np.uint32(nargs))
+            if n:
+                sds.append(p.source_digests[:n])
+            nbytes += end
+            nargs += len(p.args_offsets) - 1
+        blob = np.concatenate(blobs) if nbytes else np.zeros(1, dtype=np.uint8)
+        sd = np.concatenate(sds) if sds else parts[0].source_digests[:0]
+        return cls(blob, np.concatenate(offs), np.ascontiguousarray(np.concatenate(idx), dtype=np.uint32),
+                   np.ascontiguousarray(sd))
+
     def struct(self) -> "_abi.yd_task_sources":
         sd = self.source_digests
         return _abi.yd_task_sources(self.args.ctypes.data, self.args_offsets.ctypes.data, len(self.args_offsets) - 1,
@@ -531,6 +552,10 @@ class TaskDispatcher:
         """BASELINE configs[3] in one call (yd_filter_and_wait_for_starting_new_tasks): bloom pre-filter on the
         cache keys, in-flight dedupe on the task digests, then the solve over what is left.  Returns
         (verdicts uint8[n], hits RUNNING_HIT[n], grants GRANT[n_offered])."""
+        return self._filter_with(self._lib.yd_filter_and_wait_for_starting_new_tasks, reqs, cache_keys, task_digests, now,
+                                 out, verdict_out, want_hits)
+
+    def _filter_with(self, fn, reqs, cache_keys, task_digests, now, out, verdict_out, want_hits):
         assert reqs.dtype == REQ_DTYPE and reqs.flags.c_contiguous
         n = reqs.shape[0]
         f = _abi.yd_prefilter()
@@ -549,9 +574,10 @@ class TaskDispatcher:
         if out is None:
             out = np.zeros(max(n, 1), dtype=GRANT_DTYPE)
         assert out.dtype == GRANT_DTYPE and out.shape[0] >= n and out.flags.c_contiguous
-        k = self._lib.yd_filter_and_wait_for_starting_new_tasks(self._h, _ns(now), reqs.ctypes.data, n, C.byref(f),
-                                                                verdict.ctypes.data, hits.ctypes.data if want_hits else None,
-                                                                out.ctypes.data)
+        k = fn(self._h, _ns(now), reqs.ctypes.data, n, C.byref(f), verdict.ctypes.data,
+               hits.ctypes.data if want_hits else None, out.ctypes.data)
+        if k == C.c_size_t(-1).value:
+            raise RuntimeError("the pre-filtered solve was refused (a range-sharded group: capacities above 8192 per servant)")
         return verdict, hits, out[: int(k)]
 
     # -- cache keys and task digests from task descriptors (yd_derive_task_keys) --------------
@@ -577,6 +603,10 @@ class TaskDispatcher:
         """filter_and_wait_for_starting_new_tasks with the cache keys and task digests derived from `src`
         (yd_derive_filter_and_wait_for_starting_new_tasks): (verdicts, hits, grants of the offered requests).
         Raises TaskKeysError, deciding nothing, on input the call refuses."""
+        return self._derive_filter_with(self._optional_fn("yd_derive_filter_and_wait_for_starting_new_tasks"), reqs, src,
+                                        stages, now, out, verdict_out, want_hits)
+
+    def _derive_filter_with(self, fn, reqs, src, stages, now, out, verdict_out, want_hits):
         assert reqs.dtype == REQ_DTYPE and reqs.flags.c_contiguous
         n = reqs.shape[0]
         assert len(src.args_index) >= n and src.source_digests.shape[0] >= n
@@ -587,12 +617,14 @@ class TaskDispatcher:
             out = np.zeros(max(n, 1), dtype=GRANT_DTYPE)
         assert out.dtype == GRANT_DTYPE and out.shape[0] >= n and out.flags.c_contiguous
         f = src.struct()
-        k = self._optional_fn("yd_derive_filter_and_wait_for_starting_new_tasks")(
-            self._h, _ns(now), reqs.ctypes.data, n, C.byref(f), int(stages), verdict.ctypes.data,
-            hits.ctypes.data if want_hits else None, out.ctypes.data)
+        k = fn(self._h, _ns(now), reqs.ctypes.data, n, C.byref(f), int(stages), verdict.ctypes.data,
+               hits.ctypes.data if want_hits else None, out.ctypes.data)
         if k == C.c_size_t(-1).value:
             code = self._optional_fn("yd_derive_task_keys")(self._h, reqs.ctypes.data, n, C.byref(f), None, None)
-            raise TaskKeysError(code)
+            if code:
+                raise TaskKeysError(code)
+            raise RuntimeError("the pre-filtered solve was refused (a range-sharded group: another rank's descriptors, "
+                               "or capacities above 8192 per servant)")
         return verdict, hits, out[: int(k)]
 
     def running_index_entry(self, snapshot_index: int) -> RunningTask | None:

@@ -33,7 +33,8 @@ from typing import Callable, Sequence
 
 import numpy as np
 
-from ._abi import GRANT_DTYPE, REQ_DTYPE, STATUS_ENVIRONMENT_NOT_FOUND, STATUS_GRANTED
+from ._abi import (FILTER_OFFERED, GRANT_DTYPE, REQ_DTYPE, STAGE_CACHE, STAGE_DEDUPE, STATUS_ENVIRONMENT_NOT_FOUND,
+                   STATUS_GRANTED)
 from .dispatcher import Servant, TaskDispatcher
 
 
@@ -315,6 +316,62 @@ class RangeShardedDispatcher:
         if not self.native:
             return self.local.wait_for_starting_task_rpcs(rpcs, now)
         return self.local._rpcs_with(self.local._lib.yd_shard_wait_for_starting_task_rpcs, rpcs, now)
+
+    # -- the pre-filtered solve (BASELINE configs[3]): each rank filters its own range, then the group decides the
+    # concatenation of the offered ranges.  Both return this rank's (verdicts, hits, grants of its offered requests).
+    def filter_and_wait_for_starting_new_tasks(self, reqs_local: np.ndarray, cache_keys=None, task_digests=None,
+                                               now: float = 0.0):
+        """Collective TaskDispatcher.filter_and_wait_for_starting_new_tasks over the queue the ranks' ranges make:
+        cache_keys / task_digests are this rank's requests' keys (the same kinds on every rank)."""
+        if not self.native:
+            km = None if cache_keys is None else TaskDispatcher._key_matrix(cache_keys)
+            dm = None if task_digests is None else TaskDispatcher._key_matrix(task_digests)
+            parts = self._gather((np.ascontiguousarray(reqs_local), km, dm))
+
+            def keys(j):  # (None: no rank passed keys of this kind, or the whole queue is empty)
+                ms = [p[j][:len(p[0])] for p in parts if p[j] is not None and len(p[0])]
+                return np.concatenate(ms) if ms else None
+            whole = self.local.filter_and_wait_for_starting_new_tasks(np.concatenate([p[0] for p in parts]), keys(1), keys(2),
+                                                                      now)
+            return self._my_slice([len(p[0]) for p in parts], *whole)
+        return self.local._filter_with(self.local._lib.yd_shard_filter_and_wait_for_starting_new_tasks, reqs_local,
+                                       cache_keys, task_digests, now, None, None, True)
+
+    def derive_filter_and_wait_for_starting_new_tasks(self, reqs_local: np.ndarray, src_local,
+                                                      stages: int = STAGE_CACHE | STAGE_DEDUPE, now: float = 0.0):
+        """Collective TaskDispatcher.derive_filter_and_wait_for_starting_new_tasks: src_local (a TaskSources with its
+        own argument table) describes this rank's range.  If any rank's descriptors are refused, every rank raises
+        (TaskKeysError on the ranks whose own descriptors were refused) and nothing is decided."""
+        from .dispatcher import TaskKeysError, TaskSources
+
+        if not self.native:
+            parts = self._gather((np.ascontiguousarray(reqs_local), src_local))
+            counts = [len(p[0]) for p in parts]
+            try:
+                whole = self.local.derive_filter_and_wait_for_starting_new_tasks(
+                    np.concatenate([p[0] for p in parts]), TaskSources.concat([p[1] for p in parts], counts), stages, now)
+            except TaskKeysError:
+                # this rank's own descriptors refused: raises TaskKeysError with its code
+                self.local.derive_task_keys(reqs_local, src_local, cache_keys=False, task_digests=False)
+                raise RuntimeError("the pre-filtered solve was refused: another rank's descriptors") from None
+            return self._my_slice(counts, *whole)
+        return self.local._derive_filter_with(self.local._lib.yd_shard_derive_filter_and_wait_for_starting_new_tasks,
+                                              reqs_local, src_local, stages, now, None, None, True)
+
+    def _gather(self, obj) -> list:
+        import torch.distributed as dist
+
+        parts: list = [None] * self.world
+        dist.all_gather_object(parts, obj, group=self.group)
+        return parts
+
+    def _my_slice(self, counts, verdicts, hits, grants):
+        """This rank's part of a single handle's pre-filtered solve over the concatenated queue."""
+        lo = sum(counts[: self.rank])
+        hi = lo + counts[self.rank]
+        first = int((verdicts[:lo] == FILTER_OFFERED).sum())
+        mine = int((verdicts[lo:hi] == FILTER_OFFERED).sum())
+        return verdicts[lo:hi].copy(), None if hits is None else hits[lo:hi].copy(), grants[first:first + mine].copy()
 
     def export_state(self, now: float = 0.0) -> bytes:
         """Collective.  The group's state as ONE scheduler's export (ydstate.h), the same bytes on every rank: a

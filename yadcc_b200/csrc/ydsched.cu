@@ -720,8 +720,6 @@ yd_sched* yd_create(const yd_config* cfg) {
   return s;
 }
 
-extern "C" void yd_shard_finalize(yd_sched* s);
-
 void yd_destroy(yd_sched* s) {
   if (!s) return;
   yd_shard_finalize(s);
@@ -2349,29 +2347,8 @@ static void FilterPrepare(yd_sched* s, uint32_t N, bool bloom, size_t key_span, 
   }
 }
 
-// The last step of the pre-filtered solve on a rank of a range-sharded group: the sharded solve of the `kept` requests
-// the compaction staged (of N).  Every rank enters it, also one that kept nothing.  Leaves the stats of the solve reset
-// (the solve is yd_shard_last_stats'), with decisions = N and this rank's grants.  Returns kept, or (size_t)-1 if the
-// sharded solve refused the batch (on every rank: its refusals depend on replicated state only).
-static size_t ShardSolveKept(yd_sched* s, int64_t now_ns, uint32_t N, uint32_t kept, yd_grant* grants_out) {
-  s->staged_n = kept;
-  const int rc = yd_shard_wait_for_starting_new_tasks(s, now_ns, nullptr, kept, grants_out);
-  if (kept && s->staged_n != kept) {
-    // decided through the gathered queue, which went through the staging area: compact the offered requests there again
-    yd::k_keep_scatter<<<(N + 1023) / 1024, 1024, 0, s->st>>>(s->d_freqs.as<yd_task_req>(), s->d_fverdict.as<uint8_t>(),
-                                                              s->d_ftile.as<uint32_t>(), N, s->d_reqs.as<yd_task_req>());
-    YD_CUDA_CHECK(cudaGetLastError());
-    YD_CUDA_CHECK(cudaStreamSynchronize(s->st));
-    s->staged_n = kept;
-  }
-  s->stats = yd_solve_stats{};
-  s->stats_times_pending = 0;
-  s->have_stats = true;
-  s->stats.decisions = N;
-  if (rc) return (size_t)-1;
-  for (uint32_t i = 0; i != kept; ++i) s->stats.granted += grants_out[i].status == YD_STATUS_GRANTED;
-  return kept;
-}
+// The last step of the pre-filtered solve on a rank of a range-sharded group (shard_host.inc).
+static size_t ShardSolveKept(yd_sched* s, int64_t now_ns, uint32_t N, uint32_t kept, yd_grant* grants_out);
 
 // The device part of the pre-filtered solve, from the first filter stage on: the queue is in d_freqs, the cache keys
 // (if `bloom`) in d_bloom_keys, the task digests (if `dedupe`) in d_rt_keys, and ev_f[0] has been recorded.  The solve of
@@ -2616,9 +2593,6 @@ size_t yd_derive_filter_and_wait_for_starting_new_tasks(yd_sched* s, int64_t now
 
 }  // extern "C"
 
-// ---- range-sharded queue over the GPUs of a node (include/ydshard.h) ------------------------------------
-#include "shard_host.inc"
-
 // ---- state export / import (include/ydstate.h): host side; the lease passes are in state.cuh ----------------------
 namespace {
 
@@ -2862,177 +2836,6 @@ extern "C" int yd_import_state(yd_sched* s, int64_t now_ns, const uint8_t* blob,
   return YD_STATE_OK;
 }
 
-// ---- state export / import of a range-sharded group (ydshard.h) --------------------------------------------------------
-// The replicated sections come from each rank's own image (checked equal through a hash); the leases and the
-// bookkeeper's tasks, which each live on one rank, are gathered and merged.
-namespace {
-
-uint64_t Fnv1a(const uint8_t* p, size_t n) {
-  uint64_t h = 0xcbf29ce484222325ull;
-  for (size_t i = 0; i != n; ++i) h = (h ^ p[i]) * 0x100000001b3ull;
-  return h;
-}
-
-// All-gather of `mine` (the same word count on every rank) through device scratch: every rank's words, rank-major.
-std::vector<uint32_t> GatherWords(yd_sched* s, const std::vector<uint32_t>& mine) {
-  yd_shard_ctx* c = s->shard;
-  const size_t W = (size_t)c->world, words = mine.size();
-  uint32_t* d = static_cast<uint32_t*>(StateTmp(s, words * 4 * (W + 1)));
-  YD_CUDA_CHECK(cudaMemcpyAsync(d, mine.data(), words * 4, cudaMemcpyHostToDevice, s->st));
-  YD_NCCL_CHECK(c->api, c->api->AllGather(d, d + words, words, ncclUint32, c->comm, s->st));
-  std::vector<uint32_t> all(words * W);
-  YD_CUDA_CHECK(cudaMemcpyAsync(all.data(), d + words, words * 4 * W, cudaMemcpyDeviceToHost, s->st));
-  YD_CUDA_CHECK(cudaFreeAsync(d, s->st));
-  YD_CUDA_CHECK(cudaStreamSynchronize(s->st));
-  return all;
-}
-
-void PutU64(std::vector<uint32_t>& v, uint64_t x) { v.push_back((uint32_t)x); v.push_back((uint32_t)(x >> 32)); }
-uint64_t GetU64(const uint32_t* p) { return p[0] | (uint64_t(p[1]) << 32); }
-
-// This rank's bookkeeper tasks, group by group in iteration order: u32 count, then per task its report position,
-// servant_task_id, task_grant_id and the two strings (u32 byte length, bytes), packed into u32 words.
-std::vector<uint32_t> PackBook(const yd_sched* s) {
-  std::string b;
-  auto put = [&](const void* p, size_t n) { b.append(static_cast<const char*>(p), n); };
-  auto str = [&](const std::string& x) { const uint32_t n = (uint32_t)x.size(); put(&n, 4); put(x.data(), n); };
-  for (auto&& [loc, v] : s->running) {
-    const uint32_t n = (uint32_t)v.size();
-    put(&n, 4);
-    for (auto&& t : v) {
-      put(&t.report_pos, 4); put(&t.servant_task_id, 8); put(&t.task_grant_id, 8);
-      str(t.servant_location); str(t.task_digest);
-    }
-  }
-  std::vector<uint32_t> w((b.size() + 3) / 4, 0);
-  if (!b.empty()) memcpy(w.data(), b.data(), b.size());
-  return w;
-}
-
-// The groups' tasks of every rank's packed book (W blocks of `stride` words), merged by report position.
-void MergeBooks(const std::vector<uint32_t>& all, size_t stride, uint32_t W, std::vector<ydstate::Group>* groups) {
-  std::vector<std::vector<std::pair<uint32_t, ydstate::Task>>> got(groups->size());
-  for (uint32_t r = 0; r < W; ++r) {
-    const char* p = reinterpret_cast<const char*>(all.data() + r * stride);
-    auto get = [&](void* o, size_t n) { memcpy(o, p, n); p += n; };
-    auto str = [&]() { uint32_t n; get(&n, 4); std::string x(p, n); p += n; return x; };
-    for (auto& g : got) {
-      uint32_t n;
-      get(&n, 4);
-      for (uint32_t k = 0; k != n; ++k) {
-        uint32_t pos;
-        ydstate::Task t;
-        get(&pos, 4); get(&t.servant_task_id, 8); get(&t.task_grant_id, 8);
-        t.servant_location = str();
-        t.task_digest = str();
-        g.emplace_back(pos, std::move(t));
-      }
-    }
-  }
-  for (size_t i = 0; i != got.size(); ++i) {
-    std::sort(got[i].begin(), got[i].end(), [](auto& a, auto& b) { return a.first < b.first; });
-    auto& tasks = (*groups)[i].tasks;
-    tasks.clear();
-    for (auto& pt : got[i]) tasks.push_back(std::move(pt.second));
-  }
-}
-
-}  // namespace
-
-extern "C" size_t yd_shard_export_state(yd_sched* s, int64_t now_ns, uint8_t* out, size_t cap) {
-  yd_shard_ctx* c = s ? s->shard : nullptr;
-  if (!c) return 0;
-  YD_CUDA_CHECK(cudaSetDevice(s->device));
-  cudaStream_t st = s->st;
-  const uint32_t W = (uint32_t)c->world;
-  s->SyncServantState();
-  LiveLeases L;
-  CountLiveLeases(s, &L);
-  ydstate::StateImage im = HostImage(s, now_ns);
-  // the replicated sections: the image without lease records and without the groups' tasks
-  std::vector<ydstate::Group> groups = std::move(im.groups);
-  im.groups.clear();
-  for (auto&& g : groups) im.groups.push_back(ydstate::Group{g.location, {}});
-  std::vector<uint8_t> rep(ydstate::EncodeState(im, nullptr, 0));
-  ydstate::EncodeState(im, rep.data(), rep.size());
-  const std::vector<uint32_t> book = PackBook(s);
-  // exchange 1: lease count, hash of the replicated sections, packed book length, the room this rank offers
-  std::vector<uint32_t> hdr;
-  PutU64(hdr, L.n);
-  PutU64(hdr, Fnv1a(rep.data(), rep.size()));
-  PutU64(hdr, book.size());
-  PutU64(hdr, out ? cap : 0);
-  const std::vector<uint32_t> all = GatherWords(s, hdr);
-  std::vector<unsigned long long> counts(W);
-  uint64_t n_total = 0, maxn = 0, maxbook = 0;
-  for (uint32_t r = 0; r < W; ++r) {
-    const uint32_t* h = all.data() + r * hdr.size();
-    counts[r] = GetU64(h);
-    n_total += counts[r];
-    maxn = std::max<uint64_t>(maxn, counts[r]);
-    maxbook = std::max<uint64_t>(maxbook, GetU64(h + 4));
-    if (GetU64(h + 2) != GetU64(all.data() + 2)) {
-      fprintf(stderr, "ydsched: yd_shard_export_state: rank %u's replicated state differs from rank 0's\n", r);
-      FreeLiveLeases(s, L);
-      YD_CUDA_CHECK(cudaStreamSynchronize(st));
-      return 0;
-    }
-  }
-  // exchange 2: the books, padded to the longest
-  if (maxbook) {
-    std::vector<uint32_t> mine = book;
-    mine.resize(maxbook, 0);
-    MergeBooks(GatherWords(s, mine), maxbook, W, &groups);
-  }
-  im.groups = std::move(groups);
-  im.n_leases = n_total;
-  size_t lease_off = 0;
-  const size_t size = ydstate::EncodeState(im, nullptr, 0, &lease_off);
-  bool any_room = false;
-  for (uint32_t r = 0; r < W; ++r) any_room |= GetU64(all.data() + r * hdr.size() + 6) >= size;
-  const bool write = out && cap >= size;
-  if (write) ydstate::EncodeState(im, out, cap);
-  // exchange 3 (when some rank writes the export): the lease records, padded to the longest list, merged on the device
-  if (any_room && n_total) {
-    const size_t rb = sizeof(yd::StateLease);
-    char* t = static_cast<char*>(StateTmp(s, maxn * rb * (W + 1) + n_total * rb + W * 8));
-    yd::StateLease* d_send = reinterpret_cast<yd::StateLease*>(t);
-    yd::StateLease* d_lists = d_send + maxn;
-    yd::StateLease* d_out = d_lists + maxn * W;
-    unsigned long long* d_counts = reinterpret_cast<unsigned long long*>(d_out + n_total);
-    if (L.n) WriteLiveLeases(s, L, now_ns, d_send);
-    YD_CUDA_CHECK(cudaMemcpyAsync(d_counts, counts.data(), W * 8, cudaMemcpyHostToDevice, st));
-    YD_NCCL_CHECK(c->api, c->api->AllGather(d_send, d_lists, maxn * rb / 4, ncclUint32, c->comm, st));
-    const uint64_t threads = maxn * W;
-    yd::k_state_merge<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(d_lists, maxn, d_counts, W, d_out);
-    YD_CUDA_CHECK(cudaGetLastError());
-    if (write) YD_CUDA_CHECK(cudaMemcpyAsync(out + lease_off, d_out, n_total * rb, cudaMemcpyDeviceToHost, st));
-    YD_CUDA_CHECK(cudaFreeAsync(t, st));
-  }
-  FreeLiveLeases(s, L);
-  YD_CUDA_CHECK(cudaStreamSynchronize(st));
-  return size;
-}
-
-extern "C" int yd_shard_import_state(yd_sched* s, int64_t now_ns, const uint8_t* blob, size_t len) {
-  yd_shard_ctx* c = s ? s->shard : nullptr;
-  if (!c) return YD_STATE_UNSUPPORTED;
-  YD_CUDA_CHECK(cudaSetDevice(s->device));
-  const uint32_t W = (uint32_t)c->world, R = (uint32_t)c->rank;
-  ydstate::StateImage im;
-  const int rc = CheckImport(s, blob, len, R, W, &im);
-  // every rank's verdict and the length and hash of its blob: all or nothing, and only rank 0's export is loaded
-  std::vector<uint32_t> mine{(uint32_t)rc, 0};
-  PutU64(mine, len);
-  PutU64(mine, blob ? Fnv1a(blob, len) : 0);
-  const std::vector<uint32_t> all = GatherWords(s, mine);
-  for (uint32_t r = 0; r < W; ++r) {
-    const uint32_t* v = all.data() + r * mine.size();
-    if (v[0] != YD_STATE_OK) return (int)v[0];
-    if (GetU64(v + 2) != GetU64(all.data() + 2) || GetU64(v + 4) != GetU64(all.data() + 4)) return YD_STATE_BAD_BLOB;
-  }
-  ApplyImport(s, now_ns, im, R, W);
-  return YD_STATE_OK;
-}
-
+// ---- range-sharded queue over the GPUs of a node (include/ydshard.h) ------------------------------------
+#include "shard_host.inc"
 #include "shard_calls.inc"

@@ -64,10 +64,23 @@ constexpr uint32_t kMsNp = 32, kMsPk = 36, kMsJ0 = 44, kMsJ1 = 52;
 constexpr uint32_t kMergeSkipMax = 1u << 20;  // longest run of own-servant requests walked over (then: sequential solver)
 constexpr uint32_t kMergeMaxRounds = 16;   // changed[] is indexed by round & 15
 
+// Why a component was handed back to the sequential solver: MergePlan::viol collects one bit per rule (atomicOr), so the
+// solve's debug line can name the rules that fired.  Readers only test it for non-zero.
+constexpr uint32_t kBackPend = 1;     // more pending runs than a state carries (kMergePend)
+constexpr uint32_t kBackSkip = 2;     // a run of own-servant requests longer than kMergeSkipMax
+constexpr uint32_t kBackWindow = 4;   // a record outside the gathered window (range-sharded queue)
+constexpr uint32_t kBackCheck = 8;    // a blocking pair: the last-resort rule (k_merge_check)
+constexpr uint32_t kBackClasses = 16; // more classes than the rings are provisioned for (cannot happen)
+// A chunk whose run met one of the first three ends with this in its end state's np word and the reason in the next:
+// its start state may be a wrong guess, so the component is handed back only if the chunk's run is still this one once
+// the rounds have settled.
+constexpr uint32_t kMergeDead = 0xFFFFFFFFu;
+
 struct MergePlan {
   uint32_t* bar;         // [4] grid barrier arrivals (zeroed with the rest of the scratch region)
-  uint32_t* viol;        // [n_comps] 1: the component needs the sequential solver after all
+  uint32_t* viol;        // [n_comps] kBack* mask, non-zero: the component needs the sequential solver after all
   uint32_t* changed;     // [16] chunks re-run in round r (r & 15)
+  uint32_t* dead;        // [16] blocks holding a chunk whose end state is kMergeDead after round r (r & 15)
   uint32_t* tau;         // [S] request index that took the servant's LAST slot (kNone: still free)
 };
 
@@ -265,7 +278,7 @@ __device__ uint32_t merge_run_chunk(const MergeArgs& a, MergeSmem& sm, uint2* ri
   if (b == 0 && r > 0) return 0;  // the first chunk starts from the true state: final after round 0
   const uint32_t K = a.ct.comp_ncls[comp];
   if (K > a.kcap) {  // (cannot happen: the rings are provisioned for min(32, cls_bound) classes)
-    if (lane == 0) atomicExch(a.mp.viol + comp, 1u);
+    if (lane == 0) atomicOr(a.mp.viol + comp, kBackClasses);
     return 0;
   }
   const uint32_t nrt = a.n_rank_tiles;
@@ -299,6 +312,7 @@ __device__ uint32_t merge_run_chunk(const MergeArgs& a, MergeSmem& sm, uint2* ri
     const uint32_t m0 = my_in[lane];
     const uint32_t m1 = lane < kMergeStateWords - 32 ? my_in[32 + lane] : 0u;
     if (__all_sync(0xffffffffu, p0 == m0 && p1 == m1)) return 0;  // consistent with my predecessor: nothing to do
+    if (__shfl_sync(0xffffffffu, p1, 0) == kMergeDead) return 0;  // nothing to start from (see kMergeDead)
     h = lane < K ? min(p0, n) : 0u;
     if (lane < kMergeStateWords - 32) st[32 + lane] = p1;
     __syncwarp();
@@ -312,7 +326,7 @@ __device__ uint32_t merge_run_chunk(const MergeArgs& a, MergeSmem& sm, uint2* ri
   // ---- the chunk's slots -----------------------------------------------------------------------
   uint64_t* mbar = reinterpret_cast<uint64_t*>(sm.mbar);
   uint32_t base = lb;
-  bool dead = false;
+  uint32_t dead = 0;  // kBack* reasons to hand the component back
   // Ring bookkeeping, per stream owner (lane k for class k's records, lane 0 also for the slot list): blocks below
   // `*_hi` are in the ring or on their way, blocks below `*_ok` have landed.  A step reads blocks jb and jb + 1 of a
   // stream; block jb + 2 is requested as soon as jb is reached, i.e. a whole block of progress before it is read,
@@ -419,7 +433,7 @@ __device__ uint32_t merge_run_chunk(const MergeArgs& a, MergeSmem& sm, uint2* ri
           }
         }
         __syncwarp();
-        if (__any_sync(0xffffffffu, miss)) { dead = true; break; }
+        if (__any_sync(0xffffffffu, miss)) { dead = kBackWindow; break; }
         // a slot that took a request from its own servant: the step ends before it (the one-slot step decides it)
         const uint32_t cb = __ballot_sync(0xffffffffu, my_pick != kNone && sm.a[lane] == e.x);
         if (cb) {
@@ -445,7 +459,7 @@ __device__ uint32_t merge_run_chunk(const MergeArgs& a, MergeSmem& sm, uint2* ri
               const uint2 v = ring_rq[size_t(k) * kRingRecs + ((sm.a[k] + cnt) & (kRingRecs - 1))];
               if (v.x < nbest) { nbest = v.x; npick = k; nself = v.y; }
             } else if (cnt < sm.more[k]) {
-              sm.ovf = 1;  // a request whose record was not gathered (sharded queue only)
+              sm.ovf = kBackWindow;  // a request whose record was not gathered (sharded queue only)
             }
           }
         }
@@ -454,7 +468,7 @@ __device__ uint32_t merge_run_chunk(const MergeArgs& a, MergeSmem& sm, uint2* ri
         if (!__any_sync(0xffffffffu, moved)) break;
       }
       __syncwarp();
-      if (sm.ovf) { dead = true; break; }
+      if (sm.ovf) { dead = sm.ovf; break; }
       // a lane that would serve a request from its own servant: commit the lanes before it only
       const uint32_t cb = __ballot_sync(0xffffffffu, pick < 32 && bself == e.x);
       fb = cb ? (uint32_t)__ffs(cb) - 1u : 32u;
@@ -476,28 +490,29 @@ __device__ uint32_t merge_run_chunk(const MergeArgs& a, MergeSmem& sm, uint2* ri
       const uint2 e = a.list[base];
       const uint32_t s = e.x;
       uint32_t cq = kNone, cj = 0, pidx = kNone;
-      bool ovf = false;
+      uint32_t ovf = 0;
       if (lane < K && ((e.y >> lane) & 1u)) {
         for (uint32_t p = 0; p < np; ++p) {  // runs of a class are in queue order: the first match is the earliest
           const uint32_t pk = st[kMsPk + p];
           if ((pk >> 24) == lane && (pk & 0xFFFFFFu) != s) {
-            if (st[kMsJ0 + p] >= win) { ovf = true; break; }
+            if (st[kMsJ0 + p] >= win) { ovf = kBackWindow; break; }
             cq = a.rq[rq_base + st[kMsJ0 + p]].x; pidx = p; break;
           }
         }
         if (pidx == kNone && !ovf) {
           uint32_t j = h;
           while (j < n) {
-            if (j >= win) { ovf = true; break; }
+            if (j >= win) { ovf = kBackWindow; break; }
             const uint2 v = a.rq[rq_base + j];
             if (v.y != s) { cq = v.x; break; }
             ++j;
-            if (j - h > kMergeSkipMax) { ovf = true; break; }
+            if (j - h > kMergeSkipMax) { ovf = kBackSkip; break; }
           }
           cj = j;
         }
       }
-      if (__any_sync(0xffffffffu, ovf)) { dead = true; break; }
+      dead = __reduce_or_sync(0xffffffffu, ovf);
+      if (dead) break;
       const uint32_t m = __reduce_min_sync(0xffffffffu, cq);
       if (m != kNone) {
         const uint32_t wl = (uint32_t)__ffs(__ballot_sync(0xffffffffu, cq == m)) - 1u;
@@ -524,7 +539,7 @@ __device__ uint32_t merge_run_chunk(const MergeArgs& a, MergeSmem& sm, uint2* ri
                 st[kMsPk + cur] = key; st[kMsJ0 + cur] = h; st[kMsJ1 + cur] = cj;
                 ++cur;
               } else {
-                sm.ovf = 1;
+                sm.ovf = kBackPend;
               }
             }
             h = cj + 1;
@@ -532,7 +547,7 @@ __device__ uint32_t merge_run_chunk(const MergeArgs& a, MergeSmem& sm, uint2* ri
           st[kMsNp] = cur;
         }
         __syncwarp();
-        if (sm.ovf) { dead = true; break; }
+        if (sm.ovf) { dead = sm.ovf; break; }
         np = st[kMsNp];
       }
       if (lane == 0) a.slot_pick[base] = m;
@@ -545,7 +560,8 @@ __device__ uint32_t merge_run_chunk(const MergeArgs& a, MergeSmem& sm, uint2* ri
   par_rq = rq_par; par_ls = ls_par;
   __syncwarp();
   if (dead) {  // more pending runs than a state carries / a record that was not gathered: the sequential solver decides
-    if (lane == 0) atomicExch(a.mp.viol + comp, 1u);
+    my_out[lane] = 0;
+    if (lane < kMergeStateWords - 32) my_out[32 + lane] = lane == 0 ? kMergeDead : lane == 1 ? dead : 0u;
     return 1;
   }
   for (uint32_t idx = base + lane; idx < le; idx += 32) a.slot_pick[idx] = kNone;
@@ -594,7 +610,10 @@ __global__ void __launch_bounds__(32) k_merge_solve(MergeArgs a) {
   uint32_t par_rq = 0, par_ls = 0, epoch = 0;
   // ---- rounds -----------------------------------------------------------------------------------------------
   for (uint32_t r = 0;; ++r) {
-    if (blockIdx.x == 0 && lane == 0) atomicExch(&a.mp.changed[(r + 1) & 15u], 0u);  // (nobody touches that cell during round r)
+    if (blockIdx.x == 0 && lane == 0) {  // (nobody touches these cells during round r)
+      atomicExch(&a.mp.changed[(r + 1) & 15u], 0u);
+      atomicExch(&a.mp.dead[(r + 1) & 15u], 0u);
+    }
     uint32_t ran = 0;
     for (uint32_t t = blockIdx.x; t < total; t += gridDim.x) {
       uint32_t midx, b;
@@ -603,9 +622,27 @@ __global__ void __launch_bounds__(32) k_merge_solve(MergeArgs a) {
       __syncwarp();
     }
     if (r > 0 && ran && lane == 0) atomicAdd(&a.mp.changed[r & 15u], ran);
+    // (only read after a round that re-ran nothing, in which no end state changes)
+    if (lane == 0) {
+      bool dead = false;
+      for (uint32_t t = blockIdx.x; t < total && !dead; t += gridDim.x) dead = __ldcg(a.st_out + size_t(t) * kMergeStateWords + kMsNp) == kMergeDead;
+      if (dead) atomicAdd(&a.mp.dead[r & 15u], 1u);
+    }
     merge_grid_sync(a.mp.bar, epoch, lane);
     if (r > 0 && atomicAdd(&a.mp.changed[r & 15u], 0u) == 0) {  // nothing re-ran: every start state equals its predecessor's end
       if (blockIdx.x == 0 && lane == 0 && a.diag) { a.diag[0] = r + 1; a.diag[1] = total; }
+      if (atomicAdd(&a.mp.dead[r & 15u], 0u)) {
+        // the settled chain holds chunks that could not decide their slots (the first of them started from the true
+        // state): their components go to the sequential solver
+        for (uint32_t t = blockIdx.x; t < total && lane == 0; t += gridDim.x) {
+          const uint32_t* out = a.st_out + size_t(t) * kMergeStateWords;
+          if (__ldcg(out + kMsNp) != kMergeDead) continue;
+          uint32_t midx, b;
+          merge_locate(sm, nmerge, t, midx, b);
+          atomicOr(a.mp.viol + a.ct.merge_comp[midx], __ldcg(out + kMsNp + 1));
+        }
+        merge_grid_sync(a.mp.bar, epoch, lane);
+      }
       break;
     }
     if (r > total + 2) {  // (cannot happen: after round r the first r + 1 chunks are final)
@@ -648,7 +685,7 @@ __global__ void __launch_bounds__(256) k_merge_check(MergeArgs a) {
   const uint32_t pos = a.t.comp_sv[a.t.comp_sv_off[comp] + self];
   if (a.mp.tau[pos] <= a.L.q_base + q) return;  // every slot of the own servant went to an earlier request
   if (a.sv.max_tasks[pos] != 0 && (uint32_t)a.sv.version[pos] >= a.ct.cls_mv[c] && servant_has_env(a.t, pos, a.ct.cls_env[c])) {
-    atomicExch(a.mp.viol + comp, 1u);
+    atomicOr(a.mp.viol + comp, kBackCheck);
   }
 }
 

@@ -856,9 +856,20 @@ yd::MergePlan MakeMergePlan(yd_sched* s) {
   yd::MergePlan mp{};
   mp.bar = u;                            u += yd::kMaxClasses + 1;  // (only the first cell is used)
   mp.changed = u;                        u += 16;
+  mp.dead = u;                           u += 16;
   mp.viol = u;                           u += s->n_comps;
   mp.tau = u;                            // [S]
   return mp;
+}
+
+// What the merge solver handed back in the last solve, for the YDSCHED_DEBUG lines: the OR of the components' yd::kBack*
+// reasons, and how many components.  (Reads the scratch region: after the solve's sync, before the next solve.)
+std::pair<uint32_t, uint32_t> MergeBack(yd_sched* s) {
+  std::vector<uint32_t> viol(s->n_comps);
+  YD_CUDA_CHECK(cudaMemcpy(viol.data(), MakeMergePlan(s).viol, viol.size() * 4, cudaMemcpyDeviceToHost));
+  std::pair<uint32_t, uint32_t> r{0, 0};
+  for (uint32_t v : viol) { r.first |= v; r.second += v != 0; }
+  return r;
 }
 
 // Row-total mailboxes of the two row-parallel scans (k_scan_rows), in the zeroed scratch region.
@@ -1024,7 +1035,7 @@ void PrepareStreamBuffers(yd_sched* s, uint32_t Nb, size_t slot_b) {
   s->z_cls_off = off;
   off += (yd::kClsTableSize + 8 + 7 * yd::kMaxClasses + 3 * size_t(s->n_comps) + 32 * size_t(s->cls_bound) + 8) * 4;
   s->z_merge_off = off;
-  off += (yd::kMaxClasses + 1 + 16 + size_t(s->n_comps) + s->sv.size() + 8) * 4;
+  off += (yd::kMaxClasses + 1 + 32 + size_t(s->n_comps) + s->sv.size() + 8) * 4;
   s->z_layout_off = off;
   off += (4 * yd::kMaxClasses + 8) * 4;
   off = (off + 7) & ~size_t(7);
@@ -1779,12 +1790,13 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
     const bool have_work = S && s->n_comps;
     const uint32_t solver = plan.solver;
     const uint32_t final_path = (IsSolo(plan.variant) && have_work && solver == 2) ? 0u : (solver == 2 && have_work && nb <= 2048) ? 1u : 3u;
+    const auto back = solver == 2 && have_work && !IsSolo(plan.variant) ? MergeBack(s) : std::pair<uint32_t, uint32_t>{0, 0};
     fprintf(stderr, "ydsched: solve n %u tiny 0 variant %u order_static %d wide %d Nb %u slot_b %zu cls_bound %u final %u "
             "emask %d max_comp %zu solver %u graph %d merge_rounds %llu merge_chunks %llu walks %llu windows %llu "
-            "spec %u ring_cap %llu ring_lo %llu solve_ms %.3f\n",
+            "merge_back %u merge_back_n %u spec %u ring_cap %llu ring_lo %llu solve_ms %.3f\n",
             N, (unsigned)plan.variant, (int)(solver == 2 && s->order_static), (int)s->wide, Nb, slot_b, s->cls_bound, final_path,
             (int)s->emask_ok, (size_t)s->max_comp_servants, solver, (int)graphed, c->pad[0], c->pad[1], c->pad[2],
-            c->pad[3], spec, (unsigned long long)s->ring_cap, (unsigned long long)s->lo, stt.solve_ms);
+            c->pad[3], back.first, back.second, spec, (unsigned long long)s->ring_cap, (unsigned long long)s->lo, stt.solve_ms);
   }
 }
 }  // namespace

@@ -57,6 +57,19 @@ void yd_shard_finalize(yd_sched* s);
 int yd_shard_wait_for_starting_new_tasks(yd_sched* s, int64_t now_ns, const yd_task_req* reqs_local, size_t n_local,
                                          yd_grant* out_local);
 
+/* Collective: the same call over the packed interface (yd_wait_for_starting_new_tasks_packed, ydsched.h): 16-byte
+ * requests up and 8-byte grants down on every rank.  It is yd_shard_wait_for_starting_new_tasks on the unpacked
+ * requests (yd_unpack_req) -- the same queue, the same four exchanges, the same decisions -- with the grants packed:
+ * out_local[i] belongs to the i-th request of this rank's range, and its ordinal counts the grants of the WHOLE group's
+ * batch in FIFO order, so yd_unpack_grant(out_local[i], *ids) is, field for field, what the unpacked call returns for
+ * that request.  *ids (may be NULL) is the same on every rank, the group batch's first task id and the stride, and is
+ * valid even if nothing was granted.  reqs_local == NULL: the range staged with yd_stage_requests (24-byte records),
+ * decided with packed grants; afterwards the staging area follows the unpacked call's rules.  Returns 0; 1 (on every
+ * rank, nothing decided, no state changed) where the unpacked call refuses, and if the group's queue -- the ranges'
+ * lengths summed, known after the first exchange -- is longer than 2^30 requests (the ordinal has 30 bits). */
+int yd_shard_wait_for_starting_new_tasks_packed(yd_sched* s, int64_t now_ns, const yd_task_req16* reqs_local,
+                                                size_t n_local, yd_grant8* out_local, yd_packed_ids* ids);
+
 /* Collective FreeTask x n (task_dispatcher.cc:167-188): every rank passes the ids IT wants freed (any
  * subset, also none, also ids another rank holds); the ids are gathered, a lease is released by the rank
  * that holds it and the running_tasks decrements reach every replica through one all-reduce. */

@@ -277,9 +277,9 @@ def load_library(path: os.PathLike | str | None = None) -> C.CDLL:
         if fn is not None:
             fn.restype = restype
             fn.argtypes = argtypes
-    # include/ydshard.h: only the CUDA library has the range-sharded multi-GPU path
+    # include/ydshard.h: only the CUDA library has the range-sharded multi-GPU path (the product library must export all of it)
     for name, restype, argtypes in SHARD_PROTOTYPES:
-        fn = getattr(lib, name, None)
+        fn = getattr(lib, name) if path is None else getattr(lib, name, None)
         if fn is not None:
             fn.restype = restype
             fn.argtypes = argtypes
@@ -307,6 +307,7 @@ SHARD_PROTOTYPES = [
     ("yd_shard_init", C.c_int, [_P, C.c_int, C.c_int, _P]),
     ("yd_shard_finalize", None, [_P]),
     ("yd_shard_wait_for_starting_new_tasks", C.c_int, [_P, C.c_int64, _P, C.c_size_t, _P]),
+    ("yd_shard_wait_for_starting_new_tasks_packed", C.c_int, [_P, C.c_int64, _P, C.c_size_t, _P, _P]),
     ("yd_shard_free_tasks", C.c_int, [_P, _P, C.c_size_t]),
     ("yd_shard_last_stats", C.c_int, [_P, C.POINTER(yd_shard_stats)]),
     ("yd_shard_export_state", C.c_size_t, [_P, C.c_int64, _P, C.c_size_t]),

@@ -33,8 +33,8 @@ from typing import Callable, Sequence
 
 import numpy as np
 
-from ._abi import (FILTER_OFFERED, GRANT_DTYPE, REQ_DTYPE, STAGE_CACHE, STAGE_DEDUPE, STATUS_ENVIRONMENT_NOT_FOUND,
-                   STATUS_GRANTED)
+from ._abi import (FILTER_OFFERED, GRANT8_DTYPE, GRANT_DTYPE, PACKED_IDS_DTYPE, REQ16_DTYPE, REQ_DTYPE, STAGE_CACHE,
+                   STAGE_DEDUPE, STATUS_ENVIRONMENT_NOT_FOUND, STATUS_GRANTED)
 from .dispatcher import Servant, TaskDispatcher
 
 
@@ -269,6 +269,37 @@ class RangeShardedDispatcher:
         if rc != 0:
             raise RuntimeError(f"yd_shard_wait_for_starting_new_tasks failed: {rc}")
         return out[:n]
+
+    def wait_for_starting_new_tasks_packed(self, reqs16_local, now: float, out=None):
+        """Collective, over the packed interface (yd_shard_wait_for_starting_new_tasks_packed): reqs16_local is this
+        rank's FIFO range (REQ16_DTYPE, `pack_requests`), or an int n = the first n staged requests (24-byte records,
+        TaskDispatcher.stage_requests).  Returns (GRANT8 array, PACKED_IDS record) as
+        TaskDispatcher.wait_for_starting_new_tasks_packed(unpack=False) does; the ordinals count the grants of the
+        whole group's batch, so `unpack_grants` gives what wait_for_starting_new_tasks returns."""
+        from .dispatcher import _ns
+
+        lib, h = self.local._lib, self.local._h
+        if not self.native:
+            import torch.distributed as dist
+
+            parts: list = [None] * self.world
+            dist.all_gather_object(parts, np.ascontiguousarray(reqs16_local), group=self.group)
+            lo = sum(len(p) for p in parts[: self.rank])
+            g8, ids = self.local.wait_for_starting_new_tasks_packed(np.concatenate(parts), now, unpack=False)
+            return g8[lo:lo + len(reqs16_local)].copy(), ids
+        if isinstance(reqs16_local, (int, np.integer)):
+            n, ptr = int(reqs16_local), None
+        else:
+            assert reqs16_local.dtype == REQ16_DTYPE and reqs16_local.flags.c_contiguous
+            n, ptr = reqs16_local.shape[0], reqs16_local.ctypes.data
+        if out is None:
+            out = np.zeros(max(n, 1), dtype=GRANT8_DTYPE)
+        assert out.dtype == GRANT8_DTYPE and out.shape[0] >= n and out.flags.c_contiguous
+        ids = np.zeros(1, dtype=PACKED_IDS_DTYPE)
+        rc = lib.yd_shard_wait_for_starting_new_tasks_packed(h, _ns(now), ptr, n, out.ctypes.data, ids.ctypes.data)
+        if rc != 0:
+            raise RuntimeError(f"yd_shard_wait_for_starting_new_tasks_packed failed: {rc}")
+        return out[:n], ids[0]
 
     def free_tasks(self, ids) -> None:
         """Collective FreeTask: every rank passes the ids it wants released (its own grants, typically)."""

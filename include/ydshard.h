@@ -27,6 +27,7 @@
 #ifndef YDSHARD_H_
 #define YDSHARD_H_
 
+#include "ydfilter_packed.h"
 #include "ydkeys.h"
 #include "ydsched.h"
 #include "ydservice.h"
@@ -178,6 +179,16 @@ size_t yd_shard_derive_filter_and_wait_for_starting_new_tasks(yd_sched* s, int64
                                                               size_t n_local, const yd_task_sources* src_local,
                                                               uint32_t stages, uint8_t* verdict_out,
                                                               yd_running_hit* hits_out, yd_grant* grants_out);
+/* The same over the packed interface (yd_filter_and_wait_for_starting_new_tasks_packed, ydsched.h): defined as
+ * yd_shard_filter_and_wait_for_starting_new_tasks on the unpacked requests and the hex-expanded keys, with the grants
+ * packed as yd_shard_wait_for_starting_new_tasks_packed packs them: their ordinals count the grants of the group's whole
+ * offered queue, and *ids (may be NULL) is the same on every rank and valid even if nothing was offered.  Its refusals
+ * are the unpacked call's, and a group queue of offered requests above 2^30 (the packed solve's); each returns
+ * (size_t)-1 on every rank.  On a handle that has not joined a group, this is the single-handle call. */
+size_t yd_shard_filter_and_wait_for_starting_new_tasks_packed(yd_sched* s, int64_t now_ns, const yd_task_req16* reqs_local,
+                                                              size_t n_local, const yd_prefilter_packed* filter,
+                                                              uint8_t* verdict_out, yd_running_hit* hits_out,
+                                                              yd_grant8* grants_out, yd_packed_ids* ids);
 
 /* Device time (ms, CUDA events on the solve stream) of the last sharded solve's phases: local kernels and
  * the four exchanges.  Returns 0 if there was none. */

@@ -28,4 +28,4 @@ from ._abi import (  # noqa: F401
     load_library,
 )
 from .dispatcher import (Servant, RunningTask, TaskAllocation, TaskDispatcher, TaskKeysError, TaskSources, WaitStatus,  # noqa: F401
-                         pack_requests, unpack_grants)
+                         binary_digests, pack_requests, unpack_grants)

@@ -68,6 +68,11 @@ class yd_prefilter(C.Structure):
                 ("task_digests", C.c_void_p), ("task_digest_len", C.c_size_t), ("task_digest_stride", C.c_size_t)]
 
 
+class yd_prefilter_packed(C.Structure):
+    """The pre-filters over 32-byte binary digests: n contiguous records each, or NULL to skip the stage."""
+    _fields_ = [("cache_digests", C.c_void_p), ("task_digests", C.c_void_p)]
+
+
 FILTER_OFFERED, FILTER_CACHE_HIT, FILTER_JOINED = 0, 1, 2
 
 
@@ -277,8 +282,9 @@ def load_library(path: os.PathLike | str | None = None) -> C.CDLL:
         if fn is not None:
             fn.restype = restype
             fn.argtypes = argtypes
-    # include/ydshard.h: only the CUDA library has the range-sharded multi-GPU path (the product library must export all of it)
-    for name, restype, argtypes in SHARD_PROTOTYPES:
+    # include/ydshard.h: only the CUDA library has the range-sharded multi-GPU path; include/ydfilter_packed.h: the CPU
+    # checkers export it from builds of their own (the product library must export all of both)
+    for name, restype, argtypes in SHARD_PROTOTYPES + FILTER_PACKED_PROTOTYPES:
         fn = getattr(lib, name) if path is None else getattr(lib, name, None)
         if fn is not None:
             fn.restype = restype
@@ -322,9 +328,17 @@ SHARD_PROTOTYPES = [
     ("yd_shard_filter_and_wait_for_starting_new_tasks", C.c_size_t, [_P, C.c_int64, _P, C.c_size_t, _P, _P, _P, _P]),
     ("yd_shard_derive_filter_and_wait_for_starting_new_tasks", C.c_size_t,
      [_P, C.c_int64, _P, C.c_size_t, _P, C.c_uint32, _P, _P, _P]),
+    ("yd_shard_filter_and_wait_for_starting_new_tasks_packed", C.c_size_t,
+     [_P, C.c_int64, _P, C.c_size_t, _P, _P, _P, _P, _P]),
 ]
 
 # Every symbol include/ydstate.h declares, and its status codes.
+# include/ydfilter_packed.h: the pre-filtered solve over binary digests and packed records.
+FILTER_PACKED_PROTOTYPES = [
+    ("yd_filter_and_wait_for_starting_new_tasks_packed", C.c_size_t,
+     [_P, C.c_int64, _P, C.c_size_t, _P, _P, _P, _P, _P]),
+]
+
 # include/ydkeys.h: the task keys, exported by the CUDA library and by the checkers' builds that have them
 KEYS_PROTOTYPES = [
     ("yd_derive_task_keys", C.c_int, [_P, _P, C.c_size_t, _P, _P, _P]),

@@ -54,28 +54,60 @@ __device__ __forceinline__ unsigned long long xxh64_words(const unsigned long lo
   return h;
 }
 
+// Key loaders of k_bloom: load(i, w) writes key i into the salted buffer w from byte 4 on (the salt's 4 bytes are
+// rewritten per probe) and returns the buffer's length.
+
+// Fixed-length records: key i = keys + i * stride, key_len bytes.
+struct BloomRecords {
+  static constexpr int kWords = (kBloomMaxKey + 4 + 7) / 8;
+  const unsigned char* keys;
+  size_t stride;
+  uint32_t key_len;
+  __device__ __forceinline__ uint32_t load(uint32_t i, unsigned long long* w) const {
+    const unsigned char* k = keys + (size_t)i * stride;
+    const uint32_t total = key_len + 4;
+    const uint32_t nwords = (total + 7) / 8;
+    for (uint32_t j = 0; j < nwords; ++j) {
+      unsigned long long v = 0;
+#pragma unroll
+      for (int b = 0; b < 8; ++b) {
+        const uint32_t at = j * 8 + b;  // byte of the salted buffer
+        if (at >= 4 && at < total) v |= (unsigned long long)k[at - 4] << (8 * b);
+      }
+      w[j] = v;
+    }
+    return total;
+  }
+};
+
+// 32-byte cache digests (yd_prefilter_packed): key i = "yadcc-cxx2-entry-" + lowercase hex(digests + 32 i), 81 bytes.
+// The salted buffer is 85 bytes: salt, the prefix at bytes 4 .. 20, the hex at 21 .. 84, i.e. hex word k (characters
+// 8k .. 8k+7) straddles buffer words k + 2 (its first 3 characters, at bytes 5 .. 7) and k + 3 (the other 5).
+struct BloomCacheDigests {
+  static constexpr int kWords = 11;
+  const unsigned char* digests;
+  __device__ __forceinline__ uint32_t load(uint32_t i, unsigned long long* w) const {
+    unsigned long long h[8];
+    hex_digest(digests + (size_t)i * 32, h);
+    w[0] = 0x6364617900000000ull;  // salt | "yadc"
+    w[1] = 0x652d327878632d63ull;  // "c-cxx2-e"
+    w[2] = 0x0000002d7972746eull | (h[0] << 40);  // "ntry-"
+#pragma unroll
+    for (int k = 0; k < 8; ++k) w[k + 3] = (h[k] >> 24) | (k < 7 ? h[k + 1] << 40 : 0ull);
+    return 85;
+  }
+};
+
 // kAdd = false: PossiblyContains -> out[i]; kAdd = true: Add (atomicOr into the table).
-template <bool kAdd>
-__global__ void __launch_bounds__(128) k_bloom(const unsigned char* __restrict__ keys, uint32_t n, uint32_t key_len,
-                                               size_t stride, uint32_t num_hashes, unsigned long long mask,
+template <bool kAdd, class Keys>
+__global__ void __launch_bounds__(128) k_bloom(Keys keys, uint32_t n, uint32_t num_hashes, unsigned long long mask,
                                                uint32_t* __restrict__ table /* bytes viewed as le32 words */,
                                                uint8_t* __restrict__ out) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   // salted buffer: 4 bytes of salt, then the key
-  unsigned long long w[(kBloomMaxKey + 4 + 7) / 8];
-  const unsigned char* k = keys + (size_t)i * stride;
-  const uint32_t total = key_len + 4;
-  const uint32_t nwords = (total + 7) / 8;
-  for (uint32_t j = 0; j < nwords; ++j) {
-    unsigned long long v = 0;
-#pragma unroll
-    for (int b = 0; b < 8; ++b) {
-      const uint32_t at = j * 8 + b;  // byte of the salted buffer
-      if (at >= 4 && at < total) v |= (unsigned long long)k[at - 4] << (8 * b);
-    }
-    w[j] = v;
-  }
+  unsigned long long w[Keys::kWords];
+  const uint32_t total = keys.load(i, w);
   bool all = true;
   for (uint32_t salt = 0; salt < num_hashes; ++salt) {
     w[0] = (w[0] & 0xffffffff00000000ull) | salt;  // SaltInteger = int, little endian (:181,:201-203)

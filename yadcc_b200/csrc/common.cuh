@@ -161,6 +161,26 @@ __host__ __device__ inline uint32_t free_end(uint32_t max_tasks, uint32_t nproc,
   return max_tasks < nproc ? max_tasks : nproc;
 }
 
+// Lowercase hex of the four bytes of x (byte 0 first), as 8 characters in a little-endian word: the form in which a
+// delegate's keys carry a 32-byte digest (ydsched.h, yd_prefilter_packed).
+__device__ __forceinline__ unsigned long long hex_u32(uint32_t x) {
+  unsigned long long n = 0;  // one nibble per byte, the high nibble of each input byte first
+#pragma unroll
+  for (int b = 0; b < 4; ++b) {
+    n |= (unsigned long long)((x >> (8 * b + 4)) & 15u) << (16 * b);
+    n |= (unsigned long long)((x >> (8 * b)) & 15u) << (16 * b + 8);
+  }
+  // '0' + n, and 'a' - '0' - 10 = 39 more where n > 9 (n + 6 carries into bit 4 of its byte exactly then)
+  return n + 0x3030303030303030ull + (((n + 0x0606060606060606ull) >> 4) & 0x0101010101010101ull) * 39u;
+}
+
+// The 32-byte digest record `d` (16-byte aligned) as 8 words of its 64-character hex: h[k] = characters 8k .. 8k+7.
+__device__ __forceinline__ void hex_digest(const unsigned char* __restrict__ d, unsigned long long h[8]) {
+  const uint4 a = __ldg(reinterpret_cast<const uint4*>(d)), b = __ldg(reinterpret_cast<const uint4*>(d) + 1);
+  h[0] = hex_u32(a.x); h[1] = hex_u32(a.y); h[2] = hex_u32(a.z); h[3] = hex_u32(a.w);
+  h[4] = hex_u32(b.x); h[5] = hex_u32(b.y); h[6] = hex_u32(b.z); h[7] = hex_u32(b.w);
+}
+
 }  // namespace yd
 
 #define YD_CUDA_CHECK(expr)                                                                   \

@@ -10,7 +10,7 @@
 //
 //   k_keep_count    verdict per request (0 offered, 1 cache hit, 2 joined) + survivors per tile of 1024
 //   (k_scan_u32     exclusive scan of the tile counts, total behind them)
-//   k_keep_scatter  survivors -> the solver's queue, FIFO order kept
+//   k_keep_scatter  survivors -> the solver's queue, FIFO order kept (16-byte requests are unpacked on the way)
 #pragma once
 #include "common.cuh"
 
@@ -37,7 +37,23 @@ __global__ void __launch_bounds__(1024) k_keep_count(const uint8_t* __restrict__
   if (blockIdx.x == 0 && threadIdx.x == 0) tile_cnt[gridDim.x] = 0;  // the scan's end cell
 }
 
-__global__ void __launch_bounds__(1024) k_keep_scatter(const yd_task_req* __restrict__ in, const uint8_t* __restrict__ verdict,
+// A survivor into the solver's queue: a 24-byte request as it is, a 16-byte one (yd_task_req16) unpacked.
+__device__ __forceinline__ void keep_put(const yd_task_req* __restrict__ in, yd_task_req* __restrict__ out) {
+  const uint2* src = reinterpret_cast<const uint2*>(in);
+  uint2* dst = reinterpret_cast<uint2*>(out);
+  dst[0] = src[0]; dst[1] = src[1]; dst[2] = src[2];
+}
+__device__ __forceinline__ void keep_put(const yd_task_req16* __restrict__ in, yd_task_req* __restrict__ out) {
+  const uint4 w = *reinterpret_cast<const uint4*>(in);
+  uint2* dst = reinterpret_cast<uint2*>(out);
+  const unsigned long long ns = (unsigned long long)(w.w & 0x7fffffffu) * 1000000ull;
+  dst[0] = make_uint2(w.x, w.y);
+  dst[1] = make_uint2(w.z, (w.w & YD_LEASE_PREFETCH) ? YD_REQ_FLAG_PREFETCH : 0u);
+  dst[2] = make_uint2((uint32_t)ns, (uint32_t)(ns >> 32));
+}
+
+template <class Req>
+__global__ void __launch_bounds__(1024) k_keep_scatter(const Req* __restrict__ in, const uint8_t* __restrict__ verdict,
                                                        const uint32_t* __restrict__ tile_off, uint32_t n,
                                                        yd_task_req* __restrict__ out) {
   __shared__ uint32_t warp_cnt[32];
@@ -51,9 +67,7 @@ __global__ void __launch_bounds__(1024) k_keep_scatter(const yd_task_req* __rest
   uint32_t before = tile_off[blockIdx.x];
   for (uint32_t w = 0; w < warp; ++w) before += warp_cnt[w];
   before += __popc(bal & ((1u << lane) - 1));
-  const uint2* src = reinterpret_cast<const uint2*>(in + q);
-  uint2* dst = reinterpret_cast<uint2*>(out + before);
-  dst[0] = src[0]; dst[1] = src[1]; dst[2] = src[2];
+  keep_put(in + q, out + before);
 }
 
 }  // namespace yd

@@ -37,10 +37,25 @@ __device__ __forceinline__ unsigned long long rt_word(const unsigned char* p, ui
   return v;
 }
 
-__device__ __forceinline__ unsigned long long rt_hash(const unsigned char* p, uint32_t len) {
-  unsigned long long h = 0x9E3779B97F4A7C15ull ^ len;
-  for (uint32_t w = 0; w * 8 < len; ++w) {
-    h ^= rt_word(p, len, w);
+// A key as the index hashes and compares it: len bytes, read as little-endian 8-byte words, zero padded.
+// Fixed-length records and stored digests: bytes in memory.
+struct RtBytes {
+  const unsigned char* p;
+  uint32_t len;
+  __device__ __forceinline__ unsigned long long word(uint32_t w) const { return rt_word(p, len, w); }
+};
+// A 32-byte binary task digest (yd_prefilter_packed) as the 64-character lowercase hex it stands for, in registers.
+struct RtHex {
+  static constexpr uint32_t len = 64;
+  unsigned long long h[8];
+  __device__ __forceinline__ unsigned long long word(uint32_t w) const { return h[w]; }
+};
+
+template <class K>
+__device__ __forceinline__ unsigned long long rt_hash(const K& k) {
+  unsigned long long h = 0x9E3779B97F4A7C15ull ^ k.len;
+  for (uint32_t w = 0; w * 8 < k.len; ++w) {
+    h ^= k.word(w);
     h *= 0xff51afd7ed558ccdull;
     h ^= h >> 32;
   }
@@ -49,21 +64,40 @@ __device__ __forceinline__ unsigned long long rt_hash(const unsigned char* p, ui
   return h;
 }
 
-__device__ __forceinline__ bool rt_equal(const unsigned char* a, uint32_t la, const unsigned char* b, uint32_t lb) {
-  if (la != lb) return false;
-  for (uint32_t w = 0; w * 8 < la; ++w) {
-    if (rt_word(a, la, w) != rt_word(b, lb, w)) return false;
+template <class K>
+__device__ __forceinline__ bool rt_equal(const K& a, const RtBytes& b) {
+  if (a.len != b.len) return false;
+  for (uint32_t w = 0; w * 8 < a.len; ++w) {
+    if (a.word(w) != b.word(w)) return false;
   }
   return true;
 }
+
+// Query loaders of k_rt_find: key(q) is query q.
+// Fixed-length records: query q = keys + q * stride, key_len bytes.
+struct RtRecords {
+  const unsigned char* keys;
+  size_t stride;
+  uint32_t key_len;
+  __device__ __forceinline__ RtBytes key(uint32_t q) const { return RtBytes{keys + (size_t)q * stride, key_len}; }
+};
+// 32-byte task digests: query q = lowercase hex(digests + 32 q).  A stored digest that is not 64 bytes of lowercase hex
+// never matches.
+struct RtTaskDigests {
+  const unsigned char* digests;
+  __device__ __forceinline__ RtHex key(uint32_t q) const {
+    RtHex k;
+    hex_digest(digests + (size_t)q * 32, k.h);
+    return k;
+  }
+};
 
 // One thread per snapshot entry.
 __global__ void __launch_bounds__(256) k_rt_build(RtIndex ix, uint32_t n, uint32_t* __restrict__ distinct) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const unsigned char* key = ix.bytes + ix.off[i];
-  const uint32_t len = ix.len[i];
-  uint32_t h = (uint32_t)rt_hash(key, len) & ix.mask;
+  const RtBytes key{ix.bytes + ix.off[i], ix.len[i]};
+  uint32_t h = (uint32_t)rt_hash(key) & ix.mask;
   for (uint32_t probe = 0; probe <= ix.mask; ++probe) {
     uint32_t cur = ix.slots[h];
     if (cur == 0) {
@@ -72,7 +106,7 @@ __global__ void __launch_bounds__(256) k_rt_build(RtIndex ix, uint32_t n, uint32
     }
     // the slot belongs to some digest for good (only its entry index can grow): is it mine?
     const uint32_t o = cur - 1;
-    if (rt_equal(key, len, ix.bytes + ix.off[o], ix.len[o])) {
+    if (rt_equal(key, RtBytes{ix.bytes + ix.off[o], ix.len[o]})) {
       atomicMax(&ix.slots[h], i + 1);  // tmp[digest] = desc: the last entry wins (cc:59)
       return;
     }
@@ -81,21 +115,21 @@ __global__ void __launch_bounds__(256) k_rt_build(RtIndex ix, uint32_t n, uint32
 }
 
 // One thread per query key.
-__global__ void __launch_bounds__(256) k_rt_find(RtIndex ix, const unsigned char* __restrict__ keys, uint32_t n,
-                                                 uint32_t key_len, size_t stride,
+template <class Keys>
+__global__ void __launch_bounds__(256) k_rt_find(RtIndex ix, Keys keys, uint32_t n,
                                                  const unsigned long long* __restrict__ servant_task_id,
                                                  uint4* __restrict__ out /* yd_running_hit */) {
   const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= n) return;
-  const unsigned char* key = keys + (size_t)q * stride;
   uint4 verdict = make_uint4(0u, 0u, kNone, 0u);
   if (ix.slots != nullptr) {
-    uint32_t h = (uint32_t)rt_hash(key, key_len) & ix.mask;
+    const auto key = keys.key(q);
+    uint32_t h = (uint32_t)rt_hash(key) & ix.mask;
     for (uint32_t probe = 0; probe <= ix.mask; ++probe) {
       const uint32_t cur = ix.slots[h];
       if (cur == 0) break;
       const uint32_t o = cur - 1;
-      if (rt_equal(key, key_len, ix.bytes + ix.off[o], ix.len[o])) {
+      if (rt_equal(key, RtBytes{ix.bytes + ix.off[o], ix.len[o]})) {
         const unsigned long long id = servant_task_id[o];
         verdict = make_uint4((uint32_t)id, (uint32_t)(id >> 32), o, 1u);
         break;

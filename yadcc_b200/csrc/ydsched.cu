@@ -2206,16 +2206,16 @@ static void BloomRun(yd_sched* s, const char* keys, size_t n, size_t key_len, si
   s->d_bloom_keys.ensure(span ? span : 1);
   YD_CUDA_CHECK(cudaMemcpyAsync(s->d_bloom_keys.p, keys, span, cudaMemcpyHostToDevice, s->st));
   const unsigned grid = (unsigned)((n + 127) / 128);
+  const yd::BloomRecords recs{s->d_bloom_keys.as<unsigned char>(), stride, (uint32_t)key_len};
   if (out) {
     s->d_bloom_out.ensure(n);
-    yd::k_bloom<false><<<grid, 128, 0, s->st>>>(s->d_bloom_keys.as<unsigned char>(), (uint32_t)n, (uint32_t)key_len, stride,
-                                                s->bloom_hashes, s->bloom_bits - 1, s->d_bloom.as<uint32_t>(),
-                                                s->d_bloom_out.as<uint8_t>());
+    yd::k_bloom<false><<<grid, 128, 0, s->st>>>(recs, (uint32_t)n, s->bloom_hashes, s->bloom_bits - 1,
+                                                s->d_bloom.as<uint32_t>(), s->d_bloom_out.as<uint8_t>());
     YD_CUDA_CHECK(cudaGetLastError());
     YD_CUDA_CHECK(cudaMemcpyAsync(out, s->d_bloom_out.p, n, cudaMemcpyDeviceToHost, s->st));
   } else {
-    yd::k_bloom<true><<<grid, 128, 0, s->st>>>(s->d_bloom_keys.as<unsigned char>(), (uint32_t)n, (uint32_t)key_len, stride,
-                                               s->bloom_hashes, s->bloom_bits - 1, s->d_bloom.as<uint32_t>(), nullptr);
+    yd::k_bloom<true><<<grid, 128, 0, s->st>>>(recs, (uint32_t)n, s->bloom_hashes, s->bloom_bits - 1,
+                                               s->d_bloom.as<uint32_t>(), nullptr);
     YD_CUDA_CHECK(cudaGetLastError());
   }
   YD_CUDA_CHECK(cudaStreamSynchronize(s->st));
@@ -2324,9 +2324,9 @@ void yd_running_index_find(yd_sched* s, const char* keys, size_t n, size_t key_l
   s->d_rt_keys.ensure(span ? span : 1);
   s->d_rt_out.ensure(n * sizeof(yd_running_hit));
   YD_CUDA_CHECK(cudaMemcpyAsync(s->d_rt_keys.p, keys, span, cudaMemcpyHostToDevice, st));
-  yd::k_rt_find<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(MakeRtIndex(s), s->d_rt_keys.as<unsigned char>(), (uint32_t)n,
-                                                              (uint32_t)key_len, stride,
-                                                              s->d_rt_ids.as<unsigned long long>(), s->d_rt_out.as<uint4>());
+  yd::k_rt_find<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(
+      MakeRtIndex(s), yd::RtRecords{s->d_rt_keys.as<unsigned char>(), stride, (uint32_t)key_len}, (uint32_t)n,
+      s->d_rt_ids.as<unsigned long long>(), s->d_rt_out.as<uint4>());
   YD_CUDA_CHECK(cudaGetLastError());
   YD_CUDA_CHECK(cudaMemcpyAsync(out, s->d_rt_out.p, n * sizeof(yd_running_hit), cudaMemcpyDeviceToHost, st));
   YD_CUDA_CHECK(cudaStreamSynchronize(st));
@@ -2359,39 +2359,74 @@ static void FilterPrepare(yd_sched* s, uint32_t N, bool bloom, size_t key_span, 
   }
 }
 
-// The last step of the pre-filtered solve on a rank of a range-sharded group (shard_host.inc).
-static size_t ShardSolveKept(yd_sched* s, int64_t now_ns, uint32_t N, uint32_t kept, yd_grant* grants_out);
+// What turns the packed grants of the next batch into task ids (yd_packed_ids).
+static yd_packed_ids BatchIds(const yd_sched* s) { return yd_packed_ids{s->next_id * s->id_stride + s->id_offset, s->id_stride}; }
 
-// The device part of the pre-filtered solve, from the first filter stage on: the queue is in d_freqs, the cache keys
-// (if `bloom`) in d_bloom_keys, the task digests (if `dedupe`) in d_rt_keys, and ev_f[0] has been recorded.  The solve of
-// the compacted queue is the single handle's, or with `group` the range-sharded group's.
-static size_t FilterStages(yd_sched* s, int64_t now_ns, uint32_t N, bool bloom, size_t key_len, size_t key_stride, bool dedupe,
-                           size_t digest_len, size_t digest_stride, uint8_t* verdict_out, yd_running_hit* hits_out,
-                           yd_grant* grants_out, size_t h2d_bytes, uint32_t extra_launches, bool group) {
+// The pre-filters' keys on the device (d_bloom_keys, d_rt_keys): fixed-length records of len bytes at a stride
+// (yd_prefilter), or with `binary` contiguous 32-byte digests (yd_prefilter_packed).
+struct FilterKeys {
+  bool bloom = false, dedupe = false, binary = false;
+  size_t key_len = 0, key_stride = 0, digest_len = 0, digest_stride = 0;
+};
+
+// The compaction: the offered requests of d_freqs (24-byte records, or with `req16` 16-byte ones) -> the solver's queue.
+static void KeepScatter(yd_sched* s, uint32_t N, bool req16) {
+  const uint32_t nt = (N + 1023) / 1024;
+  if (req16) {
+    yd::k_keep_scatter<<<nt, 1024, 0, s->st>>>(s->d_freqs.as<yd_task_req16>(), s->d_fverdict.as<uint8_t>(),
+                                               s->d_ftile.as<uint32_t>(), N, s->d_reqs.as<yd_task_req>());
+  } else {
+    yd::k_keep_scatter<<<nt, 1024, 0, s->st>>>(s->d_freqs.as<yd_task_req>(), s->d_fverdict.as<uint8_t>(),
+                                               s->d_ftile.as<uint32_t>(), N, s->d_reqs.as<yd_task_req>());
+  }
+}
+
+// The last step of the pre-filtered solve on a rank of a range-sharded group (shard_host.inc).
+static size_t ShardSolveKept(yd_sched* s, int64_t now_ns, uint32_t N, uint32_t kept, bool req16, yd_grant* grants_out,
+                             yd_grant8* out8, yd_packed_ids* ids);
+
+// The device part of the pre-filtered solve, from the first filter stage on: the queue is in d_freqs (16-byte records if
+// `req16`), the keys `k` in d_bloom_keys / d_rt_keys, and ev_f[0] has been recorded.  The solve of the compacted queue is
+// the single handle's, or with `group` the range-sharded group's; its grants go to grants_out, or packed with *ids to
+// out8.
+static size_t FilterStages(yd_sched* s, int64_t now_ns, uint32_t N, const FilterKeys& k, bool req16, uint8_t* verdict_out,
+                           yd_running_hit* hits_out, yd_grant* grants_out, yd_grant8* out8, yd_packed_ids* ids,
+                           size_t h2d_bytes, uint32_t extra_launches, bool group) {
   cudaStream_t st = s->st;
   const size_t n = N;
   const uint32_t nt = (N + 1023) / 1024;
-  if (bloom) {
-    yd::k_bloom<false><<<(N + 127) / 128, 128, 0, st>>>(s->d_bloom_keys.as<unsigned char>(), N, (uint32_t)key_len,
-                                                        key_stride, s->bloom_hashes, s->bloom_bits - 1,
-                                                        s->d_bloom.as<uint32_t>(), s->d_bloom_out.as<uint8_t>());
+  if (k.bloom) {
+    unsigned char* keys = s->d_bloom_keys.as<unsigned char>();
+    if (k.binary) {
+      yd::k_bloom<false><<<(N + 127) / 128, 128, 0, st>>>(yd::BloomCacheDigests{keys}, N, s->bloom_hashes, s->bloom_bits - 1,
+                                                          s->d_bloom.as<uint32_t>(), s->d_bloom_out.as<uint8_t>());
+    } else {
+      yd::k_bloom<false><<<(N + 127) / 128, 128, 0, st>>>(yd::BloomRecords{keys, k.key_stride, (uint32_t)k.key_len}, N,
+                                                          s->bloom_hashes, s->bloom_bits - 1, s->d_bloom.as<uint32_t>(),
+                                                          s->d_bloom_out.as<uint8_t>());
+    }
   }
-  if (dedupe) {
-    yd::k_rt_find<<<(N + 255) / 256, 256, 0, st>>>(MakeRtIndex(s), s->d_rt_keys.as<unsigned char>(), N,
-                                                   (uint32_t)digest_len, digest_stride,
-                                                   s->d_rt_ids.as<unsigned long long>(), s->d_rt_out.as<uint4>());
+  if (k.dedupe) {
+    unsigned char* keys = s->d_rt_keys.as<unsigned char>();
+    if (k.binary) {
+      yd::k_rt_find<<<(N + 255) / 256, 256, 0, st>>>(MakeRtIndex(s), yd::RtTaskDigests{keys}, N,
+                                                     s->d_rt_ids.as<unsigned long long>(), s->d_rt_out.as<uint4>());
+    } else {
+      yd::k_rt_find<<<(N + 255) / 256, 256, 0, st>>>(MakeRtIndex(s), yd::RtRecords{keys, k.digest_stride, (uint32_t)k.digest_len},
+                                                     N, s->d_rt_ids.as<unsigned long long>(), s->d_rt_out.as<uint4>());
+    }
   }
-  yd::k_keep_count<<<nt, 1024, 0, st>>>(bloom ? s->d_bloom_out.as<uint8_t>() : nullptr, dedupe ? s->d_rt_out.as<uint4>() : nullptr, N,
-                                        s->d_fverdict.as<uint8_t>(), s->d_ftile.as<uint32_t>());
+  yd::k_keep_count<<<nt, 1024, 0, st>>>(k.bloom ? s->d_bloom_out.as<uint8_t>() : nullptr,
+                                        k.dedupe ? s->d_rt_out.as<uint4>() : nullptr, N, s->d_fverdict.as<uint8_t>(),
+                                        s->d_ftile.as<uint32_t>());
   yd::k_scan_u32<<<1, 1024, 0, st>>>(s->d_ftile.as<uint32_t>(), nt + 1, nullptr, 0, nullptr, 0);
-  yd::k_keep_scatter<<<nt, 1024, 0, st>>>(s->d_freqs.as<yd_task_req>(), s->d_fverdict.as<uint8_t>(), s->d_ftile.as<uint32_t>(), N,
-                                          s->d_reqs.as<yd_task_req>());
+  KeepScatter(s, N, req16);
   YD_CUDA_CHECK(cudaGetLastError());
   YD_CUDA_CHECK(cudaEventRecord(s->ev_f[1], st));
   YD_CUDA_CHECK(cudaMemcpyAsync(s->h_fcount.p, s->d_ftile.as<uint32_t>() + nt, 4, cudaMemcpyDeviceToHost, st));
   YD_CUDA_CHECK(cudaMemcpyAsync(verdict_out, s->d_fverdict.p, N, cudaMemcpyDeviceToHost, st));
   if (hits_out) {
-    if (dedupe) YD_CUDA_CHECK(cudaMemcpyAsync(hits_out, s->d_rt_out.p, n * sizeof(yd_running_hit), cudaMemcpyDeviceToHost, st));
+    if (k.dedupe) YD_CUDA_CHECK(cudaMemcpyAsync(hits_out, s->d_rt_out.p, n * sizeof(yd_running_hit), cudaMemcpyDeviceToHost, st));
     else for (size_t i = 0; i != n; ++i) hits_out[i] = yd_running_hit{0, YD_NO_SERVANT, 0};
   }
   YD_CUDA_CHECK(cudaStreamSynchronize(st));
@@ -2400,14 +2435,15 @@ static size_t FilterStages(yd_sched* s, int64_t now_ns, uint32_t N, bool bloom, 
   cudaEventElapsedTime(&filter_ms, s->ev_f[0], s->ev_f[1]);
   size_t ret = kept;
   if (group) {
-    ret = ShardSolveKept(s, now_ns, N, kept, grants_out);
+    ret = ShardSolveKept(s, now_ns, N, kept, req16, grants_out, out8, ids);
     s->stats.total_ms = filter_ms;
   } else if (kept) {
     s->staged_n = kept;  // the compaction wrote the solver's queue
-    WaitImpl(s, now_ns, nullptr, nullptr, kept, grants_out, nullptr, nullptr);
+    WaitImpl(s, now_ns, nullptr, nullptr, kept, grants_out, out8, ids);
     yd_solve_stats st2;
     yd_last_solve_stats(s, &st2);  // (turns the solve's events into milliseconds before they are reused)
   } else {
+    if (ids) *ids = BatchIds(s);
     s->stats = yd_solve_stats{};
     s->stats_times_pending = 0;
     s->have_stats = true;
@@ -2415,44 +2451,73 @@ static size_t FilterStages(yd_sched* s, int64_t now_ns, uint32_t N, bool bloom, 
   // stats of the whole call: prep = the filter stages + compaction (device), solve / final = the solve's, decisions = n
   s->stats.prep_ms += filter_ms;
   s->stats.decisions = N;
-  s->stats.kernel_launches += 3 + (bloom ? 1 : 0) + (dedupe ? 1 : 0) + extra_launches;
+  s->stats.kernel_launches += 3 + (k.bloom ? 1 : 0) + (k.dedupe ? 1 : 0) + extra_launches;
   s->stats.h2d_bytes += h2d_bytes;
-  s->stats.d2h_bytes += N + 4 + (hits_out && dedupe ? n * sizeof(yd_running_hit) : 0);
+  s->stats.d2h_bytes += N + 4 + (hits_out && k.dedupe ? n * sizeof(yd_running_hit) : 0);
   return ret;
 }
 
 // BASELINE configs[3] in one call: bloom probes, in-flight index probes, order-preserving compaction and the solve,
-// with the queue resident in HBM from the first stage to the last (filter.cuh).  `group`: the solve is the range-sharded
-// group's (yd_shard_filter_and_wait_for_starting_new_tasks).
-static size_t FilterCall(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, size_t n, const yd_prefilter* f,
-                         uint8_t* verdict_out, yd_running_hit* hits_out, yd_grant* grants_out, bool group) {
-  if (n == 0) return group ? ShardSolveKept(s, now_ns, 0, 0, grants_out) : 0;
+// with the queue resident in HBM from the first stage to the last (filter.cuh).  The requests are `reqs` (24-byte records)
+// with the keys of `f`, and the grants 16-byte records in grants_out; or, packed, `reqs16` (16-byte records) with the
+// digests of `fp`, and the grants 8-byte records in out8 with *ids.  `group`: the solve is the range-sharded group's
+// (yd_shard_filter_and_wait_for_starting_new_tasks and its packed twin).
+static size_t FilterCall(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_task_req16* reqs16, size_t n,
+                         const yd_prefilter* f, const yd_prefilter_packed* fp, uint8_t* verdict_out, yd_running_hit* hits_out,
+                         yd_grant* grants_out, yd_grant8* out8, yd_packed_ids* ids, bool group) {
+  if (n == 0) {
+    if (group) return ShardSolveKept(s, now_ns, 0, 0, false, grants_out, out8, ids);
+    if (ids) *ids = BatchIds(s);
+    return 0;
+  }
   if (n > 0x40000000ull) { fprintf(stderr, "ydsched: batch too large\n"); abort(); }
   YD_CUDA_CHECK(cudaSetDevice(s->device));
   cudaStream_t st = s->st;
   const uint32_t N = (uint32_t)n;
-  const bool bloom = f && f->cache_keys, dedupe = f && f->task_digests;
-  if (bloom) {
-    if (!s->bloom_bits) { fprintf(stderr, "ydsched: bloom filter used before yd_bloom_reset / yd_bloom_load\n"); abort(); }
-    if (f->cache_key_len > yd::kBloomMaxKey) { fprintf(stderr, "ydsched: bloom keys longer than %d bytes\n", yd::kBloomMaxKey); abort(); }
+  const bool req16 = reqs16 != nullptr;
+  FilterKeys k;
+  const void *key_src = nullptr, *digest_src = nullptr;
+  if (fp) {
+    k.binary = true;
+    k.bloom = fp->cache_digests, k.dedupe = fp->task_digests;
+    key_src = fp->cache_digests, digest_src = fp->task_digests;
+  } else if (f) {
+    k.bloom = f->cache_keys, k.dedupe = f->task_digests;
+    key_src = f->cache_keys, digest_src = f->task_digests;
+    k.key_len = f->cache_key_len, k.key_stride = f->cache_key_stride;
+    k.digest_len = f->task_digest_len, k.digest_stride = f->task_digest_stride;
   }
-  const size_t key_span = bloom ? (n - 1) * f->cache_key_stride + f->cache_key_len : 0;
-  const size_t digest_span = dedupe ? (n - 1) * f->task_digest_stride + f->task_digest_len : 0;
-  FilterPrepare(s, N, bloom, key_span, dedupe, digest_span);
+  if (k.bloom) {
+    if (!s->bloom_bits) { fprintf(stderr, "ydsched: bloom filter used before yd_bloom_reset / yd_bloom_load\n"); abort(); }
+    if (k.key_len > yd::kBloomMaxKey) { fprintf(stderr, "ydsched: bloom keys longer than %d bytes\n", yd::kBloomMaxKey); abort(); }
+  }
+  const size_t key_span = !k.bloom ? 0 : k.binary ? n * 32 : (n - 1) * k.key_stride + k.key_len;
+  const size_t digest_span = !k.dedupe ? 0 : k.binary ? n * 32 : (n - 1) * k.digest_stride + k.digest_len;
+  const size_t req_bytes = size_t(N) * (req16 ? sizeof(yd_task_req16) : sizeof(yd_task_req));
+  FilterPrepare(s, N, k.bloom, key_span, k.dedupe, digest_span);
   // uploads: the queue, the cache keys, the task digests (one stream: each stage starts when its input has landed)
-  YD_CUDA_CHECK(cudaMemcpyAsync(s->d_freqs.p, reqs, size_t(N) * sizeof(yd_task_req), cudaMemcpyHostToDevice, st));
-  if (bloom) YD_CUDA_CHECK(cudaMemcpyAsync(s->d_bloom_keys.p, f->cache_keys, key_span, cudaMemcpyHostToDevice, st));
-  if (dedupe) YD_CUDA_CHECK(cudaMemcpyAsync(s->d_rt_keys.p, f->task_digests, digest_span, cudaMemcpyHostToDevice, st));
+  YD_CUDA_CHECK(cudaMemcpyAsync(s->d_freqs.p, req16 ? static_cast<const void*>(reqs16) : reqs, req_bytes,
+                                cudaMemcpyHostToDevice, st));
+  if (k.bloom) YD_CUDA_CHECK(cudaMemcpyAsync(s->d_bloom_keys.p, key_src, key_span, cudaMemcpyHostToDevice, st));
+  if (k.dedupe) YD_CUDA_CHECK(cudaMemcpyAsync(s->d_rt_keys.p, digest_src, digest_span, cudaMemcpyHostToDevice, st));
   YD_CUDA_CHECK(cudaEventRecord(s->ev_f[0], st));
-  return FilterStages(s, now_ns, N, bloom, bloom ? f->cache_key_len : 0, bloom ? f->cache_key_stride : 0, dedupe,
-                      dedupe ? f->task_digest_len : 0, dedupe ? f->task_digest_stride : 0, verdict_out, hits_out, grants_out,
-                      size_t(N) * sizeof(yd_task_req) + key_span + digest_span, 0, group);
+  return FilterStages(s, now_ns, N, k, req16, verdict_out, hits_out, grants_out, out8, ids, req_bytes + key_span + digest_span,
+                      0, group);
 }
 
 size_t yd_filter_and_wait_for_starting_new_tasks(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, size_t n,
                                                  const yd_prefilter* f, uint8_t* verdict_out, yd_running_hit* hits_out,
                                                  yd_grant* grants_out) {
-  return FilterCall(s, now_ns, reqs, n, f, verdict_out, hits_out, grants_out, false);
+  return FilterCall(s, now_ns, reqs, nullptr, n, f, nullptr, verdict_out, hits_out, grants_out, nullptr, nullptr, false);
+}
+
+size_t yd_filter_and_wait_for_starting_new_tasks_packed(yd_sched* s, int64_t now_ns, const yd_task_req16* reqs, size_t n,
+                                                        const yd_prefilter_packed* filter, uint8_t* verdict_out,
+                                                        yd_running_hit* hits_out, yd_grant8* grants_out,
+                                                        yd_packed_ids* ids) {
+  yd_packed_ids local;
+  return FilterCall(s, now_ns, nullptr, reqs, n, nullptr, filter, verdict_out, hits_out, nullptr, grants_out,
+                    ids ? ids : &local, false);
 }
 
 // ---- cache keys and task digests from task descriptors (blake3.cuh) ------------------------------------------------
@@ -2570,7 +2635,7 @@ int yd_derive_task_keys(yd_sched* s, const yd_task_req* reqs, size_t n, const yd
 static size_t DeriveFilterCall(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, size_t n, const yd_task_sources* src,
                                uint32_t stages, uint8_t* verdict_out, yd_running_hit* hits_out, yd_grant* grants_out,
                                bool group) {
-  if (n == 0) return group ? ShardSolveKept(s, now_ns, 0, 0, grants_out) : 0;
+  if (n == 0) return group ? ShardSolveKept(s, now_ns, 0, 0, false, grants_out, nullptr, nullptr) : 0;
   if (n > 0x40000000ull) { fprintf(stderr, "ydsched: batch too large\n"); abort(); }
   const bool bloom = stages & YD_STAGE_CACHE, dedupe = stages & YD_STAGE_DEDUPE;
   if (bloom && !s->bloom_bits) { fprintf(stderr, "ydsched: bloom filter used before yd_bloom_reset / yd_bloom_load\n"); abort(); }
@@ -2590,9 +2655,12 @@ static size_t DeriveFilterCall(yd_sched* s, int64_t now_ns, const yd_task_req* r
     LaunchTaskKeys(s, k.ks);
     YD_CUDA_CHECK(cudaFreeAsync(k.base, st));
   }
-  return FilterStages(s, now_ns, N, bloom, YD_KEYS_CACHE_KEY_LEN, YD_KEYS_CACHE_KEY_LEN, dedupe, YD_KEYS_TASK_DIGEST_LEN,
-                      YD_KEYS_TASK_DIGEST_LEN, verdict_out, hits_out, grants_out, size_t(N) * sizeof(yd_task_req) + k.h2d,
-                      (bloom || dedupe) ? 1u : 0u, group);
+  FilterKeys fk;
+  fk.bloom = bloom, fk.dedupe = dedupe;
+  fk.key_len = fk.key_stride = YD_KEYS_CACHE_KEY_LEN;
+  fk.digest_len = fk.digest_stride = YD_KEYS_TASK_DIGEST_LEN;
+  return FilterStages(s, now_ns, N, fk, false, verdict_out, hits_out, grants_out, nullptr, nullptr,
+                      size_t(N) * sizeof(yd_task_req) + k.h2d, (bloom || dedupe) ? 1u : 0u, group);
 }
 
 size_t yd_derive_filter_and_wait_for_starting_new_tasks(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, size_t n,

@@ -161,6 +161,28 @@ def pack_requests(reqs: np.ndarray, out: np.ndarray | None = None) -> np.ndarray
     return out
 
 
+CACHE_KEY_PREFIX = b"yadcc-cxx2-entry-"
+
+
+def binary_digests(keys) -> np.ndarray:
+    """Delegate keys -> the (n, 32) uint8 digests yd_prefilter_packed carries: 64-character lowercase hex task digests,
+    or 81-byte cache keys ("yadcc-cxx2-entry-" + 64 hex characters), as strings, bytes or an (n, 64) / (n, 81) uint8
+    matrix.  Raises ValueError on a key that is not of either form."""
+    m = TaskDispatcher._key_matrix(keys)
+    if m.shape[1] == len(CACHE_KEY_PREFIX) + 64:
+        if (m[:, :len(CACHE_KEY_PREFIX)] != np.frombuffer(CACHE_KEY_PREFIX, dtype=np.uint8)).any():
+            raise ValueError("a cache key without the yadcc-cxx2-entry- prefix")
+        m = m[:, len(CACHE_KEY_PREFIX):]
+    if m.shape[0] and m.shape[1] != 64:
+        raise ValueError(f"keys of {m.shape[1]} bytes: neither a task digest (64) nor a cache key (81)")
+    digit = (m >= ord("0")) & (m <= ord("9"))
+    lower = (m >= ord("a")) & (m <= ord("f"))
+    if not (digit | lower).all():
+        raise ValueError("a key that is not lowercase hex")
+    nib = np.where(digit, m - ord("0"), m - ord("a") + 10).astype(np.uint8)
+    return np.ascontiguousarray((nib[:, 0::2] << 4) | nib[:, 1::2]).reshape(m.shape[0], 32)
+
+
 def unpack_grants(g8: np.ndarray, ids) -> np.ndarray:
     """GRANT8 + PACKED_IDS -> GRANT_DTYPE (yd_unpack_grant)."""
     out = np.zeros(g8.shape[0], dtype=GRANT_DTYPE)
@@ -580,6 +602,43 @@ class TaskDispatcher:
             raise RuntimeError("the pre-filtered solve was refused (a range-sharded group: capacities above 8192 per servant)")
         return verdict, hits, out[: int(k)]
 
+    def filter_and_wait_for_starting_new_tasks_packed(self, reqs16: np.ndarray, cache_digests=None, task_digests=None,
+                                                      now: float = 0.0, hits: bool = False, *,
+                                                      out8: np.ndarray | None = None,
+                                                      verdict_out: np.ndarray | None = None):
+        """filter_and_wait_for_starting_new_tasks over the packed interface
+        (yd_filter_and_wait_for_starting_new_tasks_packed): 16-byte requests (`pack_requests`), the keys as (n, 32)
+        uint8 binary digests (`binary_digests`), 8-byte grants.  Returns (verdicts uint8[n], hits RUNNING_HIT[n] or
+        None, GRANT8[n_offered], PACKED_IDS record); `unpack_grants(grants8, ids)` gives the unpacked call's grants."""
+        return self._filter_packed_with(self._optional_fn("yd_filter_and_wait_for_starting_new_tasks_packed"), reqs16, cache_digests,
+                                        task_digests, now, hits, out8, verdict_out)
+
+    def _filter_packed_with(self, fn, reqs16, cache_digests, task_digests, now, want_hits, out8, verdict_out):
+        assert reqs16.dtype == _abi.REQ16_DTYPE and reqs16.flags.c_contiguous
+        n = reqs16.shape[0]
+
+        def digests(d):
+            if d is None:
+                return None
+            d = np.ascontiguousarray(d, dtype=np.uint8).reshape(-1, 32)
+            assert d.shape[0] >= n
+            return d
+        cd, td = digests(cache_digests), digests(task_digests)
+        f = _abi.yd_prefilter_packed(cd.ctypes.data if cd is not None else None, td.ctypes.data if td is not None else None)
+        verdict = verdict_out[:n] if verdict_out is not None else np.zeros(n, dtype=np.uint8)
+        assert verdict.dtype == np.uint8 and verdict.shape[0] == n and verdict.flags.c_contiguous
+        hit = np.zeros(n, dtype=_abi.RUNNING_HIT_DTYPE) if want_hits else None
+        if out8 is None:
+            out8 = np.zeros(max(n, 1), dtype=_abi.GRANT8_DTYPE)
+        assert out8.dtype == _abi.GRANT8_DTYPE and out8.shape[0] >= n and out8.flags.c_contiguous
+        ids = np.zeros(1, dtype=_abi.PACKED_IDS_DTYPE)
+        k = fn(self._h, _ns(now), reqs16.ctypes.data, n, C.byref(f), verdict.ctypes.data,
+               hit.ctypes.data if want_hits else None, out8.ctypes.data, ids.ctypes.data)
+        if k == C.c_size_t(-1).value:
+            raise RuntimeError("the pre-filtered solve was refused (a range-sharded group: capacities above 8192 per servant, "
+                               "or more than 2^30 offered requests)")
+        return verdict, hit, out8[: int(k)], ids[0]
+
     # -- cache keys and task digests from task descriptors (yd_derive_task_keys) --------------
     def derive_task_keys(self, reqs: np.ndarray, src: TaskSources, *, cache_keys: bool = True, task_digests: bool = True):
         """GetCxxCacheEntryKey / GetCxxTaskDigest for every request: ((n, 81) uint8 or None, (n, 64) uint8 or None),
@@ -637,7 +696,8 @@ class TaskDispatcher:
                            (t.task_digest or b"").decode())
 
     def _optional_fn(self, name: str):
-        """An entry point not every checker build exports (the state export / import, the task keys)."""
+        """An entry point not every checker build exports (the state export / import, the task keys, the packed
+        pre-filtered solve)."""
         fn = getattr(self._lib, name, None)
         if fn is None:
             raise NotImplementedError(f"{self._lib._yd_path} does not export {name}")

@@ -368,6 +368,25 @@ class RangeShardedDispatcher:
         return self.local._filter_with(self.local._lib.yd_shard_filter_and_wait_for_starting_new_tasks, reqs_local,
                                        cache_keys, task_digests, now, None, None, True)
 
+    def filter_and_wait_for_starting_new_tasks_packed(self, reqs16_local: np.ndarray, cache_digests=None, task_digests=None,
+                                                      now: float = 0.0, hits: bool = False):
+        """Collective TaskDispatcher.filter_and_wait_for_starting_new_tasks_packed over the queue the ranks' ranges make
+        (yd_shard_filter_and_wait_for_starting_new_tasks_packed): this rank's (verdicts, hits or None, GRANT8 of its
+        offered requests, PACKED_IDS record); the ordinals count the grants of the group's whole offered queue, and the
+        ids are the same on every rank."""
+        if not self.native:
+            digests = lambda d: None if d is None else np.ascontiguousarray(d, dtype=np.uint8).reshape(-1, 32)  # noqa: E731
+            parts = self._gather((np.ascontiguousarray(reqs16_local), digests(cache_digests), digests(task_digests)))
+
+            def keys(j):  # (None: no rank passed digests of this kind, or the whole queue is empty)
+                ms = [p[j][:len(p[0])] for p in parts if p[j] is not None and len(p[0])]
+                return np.concatenate(ms) if ms else None
+            v, h, g8, ids = self.local.filter_and_wait_for_starting_new_tasks_packed(
+                np.concatenate([p[0] for p in parts]), keys(1), keys(2), now, hits)
+            return (*self._my_slice([len(p[0]) for p in parts], v, h, g8), ids)
+        return self.local._filter_packed_with(self.local._lib.yd_shard_filter_and_wait_for_starting_new_tasks_packed,
+                                              reqs16_local, cache_digests, task_digests, now, hits, None, None)
+
     def derive_filter_and_wait_for_starting_new_tasks(self, reqs_local: np.ndarray, src_local,
                                                       stages: int = STAGE_CACHE | STAGE_DEDUPE, now: float = 0.0):
         """Collective TaskDispatcher.derive_filter_and_wait_for_starting_new_tasks: src_local (a TaskSources with its

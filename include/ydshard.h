@@ -112,6 +112,10 @@ int yd_shard_import_state(yd_sched* s, int64_t now_ns, const uint8_t* blob, size
  * id and the decrements.  Returns 0; 1 (nothing exchanged) if the handle has not joined a group or n >= 2^30. */
 int yd_shard_keep_task_alive(yd_sched* s, int64_t now_ns, const uint64_t* task_ids, size_t n, int64_t new_expires_in_ns,
                              uint8_t* ok_out);
+/* KeepTaskAlive x n with a lease length per id, as yd_keep_tasks_alive (the last occurrence of an id sets its expiry);
+ * the same one all-reduce and return values as yd_shard_keep_task_alive, which is its case of one length. */
+int yd_shard_keep_tasks_alive(yd_sched* s, int64_t now_ns, const uint64_t* task_ids, const int64_t* new_expires_in_ns,
+                              size_t n, uint8_t* ok_out);
 /* NotifyServantRunningTasks x n, as yd_notify_servants_running_tasks.  Each rank sweeps and checks its own leases; one
  * sum all-reduce of a u32 word per reported id (rank + 1 where permitted) and the decrements.  An id is unknown iff no
  * rank permits it.  Each rank's bookkeeper keeps the tasks whose lease it holds. */

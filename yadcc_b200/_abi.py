@@ -174,6 +174,20 @@ class yd_heartbeat_response(C.Structure):
     ]
 
 
+class yd_keep_task_alive_request(C.Structure):
+    _fields_ = [
+        ("token", C.c_char_p),
+        ("next_keep_alive_in_ms", C.c_uint32),
+        ("task_grant_ids", C.c_void_p),
+        ("n", C.c_size_t),
+        ("statuses", C.c_void_p),
+    ]
+
+
+class yd_free_task_request(C.Structure):
+    _fields_ = [("token", C.c_char_p), ("task_grant_ids", C.c_void_p), ("n", C.c_size_t)]
+
+
 class yd_wire_in(C.Structure):
     _fields_ = [("data", C.c_void_p), ("len", C.c_size_t), ("remote_ip", C.c_char_p), ("remote_is_ipv6", C.c_uint32),
                 ("reserved", C.c_uint32)]
@@ -282,9 +296,9 @@ def load_library(path: os.PathLike | str | None = None) -> C.CDLL:
         if fn is not None:
             fn.restype = restype
             fn.argtypes = argtypes
-    # include/ydshard.h: only the CUDA library has the range-sharded multi-GPU path; include/ydfilter_packed.h: the CPU
-    # checkers export it from builds of their own (the product library must export all of both)
-    for name, restype, argtypes in SHARD_PROTOTYPES + FILTER_PACKED_PROTOTYPES:
+    # include/ydshard.h: only the CUDA library has the range-sharded multi-GPU path; include/ydfilter_packed.h and
+    # include/ydruns.h: the CPU checkers export them from builds of their own (the product library must export all)
+    for name, restype, argtypes in SHARD_PROTOTYPES + FILTER_PACKED_PROTOTYPES + RUNS_PROTOTYPES:
         fn = getattr(lib, name) if path is None else getattr(lib, name, None)
         if fn is not None:
             fn.restype = restype
@@ -319,6 +333,7 @@ SHARD_PROTOTYPES = [
     ("yd_shard_export_state", C.c_size_t, [_P, C.c_int64, _P, C.c_size_t]),
     ("yd_shard_import_state", C.c_int, [_P, C.c_int64, _P, C.c_size_t]),
     ("yd_shard_keep_task_alive", C.c_int, [_P, C.c_int64, _P, C.c_size_t, C.c_int64, _P]),
+    ("yd_shard_keep_tasks_alive", C.c_int, [_P, C.c_int64, _P, _P, C.c_size_t, _P]),
     ("yd_shard_notify_servants_running_tasks", C.c_size_t,
      [_P, C.POINTER(yd_heartbeat_item), C.c_size_t, C.POINTER(C.c_uint64), C.POINTER(C.c_size_t)]),
     ("yd_shard_get_running_tasks", C.c_size_t, [_P, C.POINTER(yd_running_task), C.c_size_t]),
@@ -363,6 +378,16 @@ SERVICE_PROTOTYPES = [
     ("yd_service_keep_task_alive", C.c_int, [_P, C.c_int64, C.c_char_p, C.c_uint32, _P, C.c_size_t, _P]),
     ("yd_service_free_task", C.c_int, [_P, C.c_char_p, _P, C.c_size_t]),
     ("yd_service_get_running_tasks", C.c_size_t, [_P, C.POINTER(yd_running_task), C.c_size_t]),
+]
+
+# include/ydruns.h: runs of Heartbeat, KeepTaskAlive and FreeTask RPCs as one batch each, and KeepTaskAlive with a lease
+# length per id.
+RUNS_PROTOTYPES = [
+    ("yd_keep_tasks_alive", None, [_P, C.c_int64, _P, _P, C.c_size_t, _P]),
+    ("yd_service_heartbeats", None,
+     [_P, C.c_int64, C.POINTER(yd_heartbeat_request), C.c_size_t, C.POINTER(yd_heartbeat_response), C.POINTER(C.c_int)]),
+    ("yd_service_keep_tasks_alive", None, [_P, C.c_int64, C.POINTER(yd_keep_task_alive_request), C.c_size_t, C.POINTER(C.c_int)]),
+    ("yd_service_free_tasks", None, [_P, C.POINTER(yd_free_task_request), C.c_size_t, C.POINTER(C.c_int)]),
 ]
 
 # Every symbol include/ydwire.h declares.

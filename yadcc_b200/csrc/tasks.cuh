@@ -299,9 +299,13 @@ __global__ void k_free(const unsigned long long* __restrict__ ids, uint32_t n, T
 
 // ---- KeepTaskAlive (cc:142-165) ----------------------------------------------
 // `ok` is bytes for one handle, u32 words for a range-sharded group (the words travel in a sum all-reduce).
+// `lens` == null: every id gets `new_expires_in_ns`.  Otherwise id i gets lens[i], and only the id's last occurrence in
+// the array (last[i] != 0, marked by the host) writes the expiry, so that the last length wins as in the loop of single
+// calls.  The answer depends on the lease's flags alone, which this kernel does not change: every occurrence gets it.
 template <typename Flag>
 __global__ void k_keep_alive(const unsigned long long* __restrict__ ids, uint32_t n, long long now_ns,
-                             long long new_expires_in_ns, TaskRing ring, Flag* __restrict__ ok) {
+                             long long new_expires_in_ns, const long long* __restrict__ lens,
+                             const uint8_t* __restrict__ last, TaskRing ring, Flag* __restrict__ ok) {
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   unsigned long long id;
@@ -310,7 +314,8 @@ __global__ void k_keep_alive(const unsigned long long* __restrict__ ids, uint32_
     uint64_t slot = id & ring.mask;
     uint32_t f = ring.flags[slot];
     if ((f & kTaskAlive) && !(f & kTaskZombie)) {
-      ring.exp[slot] = now_ns + new_expires_in_ns;
+      if (!lens) ring.exp[slot] = now_ns + new_expires_in_ns;
+      else if (last[i]) ring.exp[slot] = now_ns + lens[i];
       r = 1;
     }
   }

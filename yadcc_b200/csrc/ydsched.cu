@@ -22,6 +22,7 @@
 #include <type_traits>
 #include <string>
 #include <unordered_map>
+#include <unordered_set>
 #include <vector>
 
 #include "common.cuh"
@@ -42,6 +43,7 @@
 #include "ydstate_codec.inc"
 #include "ydkeys.h"
 #include "ydshard.h"
+#include "ydruns.h"
 #include "ydsched_keys_impl.inc"
 
 namespace {
@@ -1815,20 +1817,66 @@ void yd_wait_for_starting_new_tasks_packed(yd_sched* s, int64_t now_ns, const yd
   WaitImpl(s, now_ns, nullptr, reqs, n, nullptr, out, ids ? ids : &local);
 }
 
+extern "C++" {
+namespace {
+// KeepTaskAlive's upload to d_ids, then k_keep_alive writing `ok` (n flags of type Flag, on the device).  With one length
+// (`lens` == null) the ids go up as they are.  With a length per id, the ids, the lengths and each id's last-occurrence
+// mark go up in one copy; if the lengths are all equal this is the one-length call.
+template <typename Flag>
+void KeepAlive(yd_sched* s, int64_t now_ns, const uint64_t* ids, const int64_t* lens, size_t n, int64_t new_expires_in_ns,
+               Flag* ok) {
+  if (lens && std::all_of(lens, lens + n, [&](int64_t x) { return x == lens[0]; })) {
+    new_expires_in_ns = lens[0];
+    lens = nullptr;
+  }
+  const long long* d_lens = nullptr;
+  const uint8_t* d_last = nullptr;
+  if (!lens) {
+    s->d_ids.ensure(n * 8);
+    YD_CUDA_CHECK(cudaMemcpyAsync(s->d_ids.p, ids, n * 8, cudaMemcpyHostToDevice, s->st));
+  } else {
+    const size_t bytes = n * 17;  // ids (u64) | lengths (i64) | last-occurrence marks (u8)
+    s->h_small.ensure(bytes);
+    char* h = s->h_small.as<char>();
+    memcpy(h, ids, n * 8);
+    memcpy(h + n * 8, lens, n * 8);
+    uint8_t* last = reinterpret_cast<uint8_t*>(h + n * 16);
+    std::unordered_set<uint64_t> seen;
+    seen.reserve(n);
+    for (size_t i = n; i-- > 0;) last[i] = seen.insert(ids[i]).second ? 1 : 0;
+    s->d_ids.ensure(bytes);
+    YD_CUDA_CHECK(cudaMemcpyAsync(s->d_ids.p, h, bytes, cudaMemcpyHostToDevice, s->st));
+    d_lens = reinterpret_cast<const long long*>(s->d_ids.as<char>() + n * 8);
+    d_last = reinterpret_cast<const uint8_t*>(s->d_ids.as<char>() + n * 16);
+  }
+  yd::k_keep_alive<<<(unsigned)((n + 255) / 256), 256, 0, s->st>>>(s->d_ids.as<unsigned long long>(), (uint32_t)n,
+                                                                    (long long)now_ns, (long long)new_expires_in_ns,
+                                                                    d_lens, d_last, s->ring(), ok);
+  YD_CUDA_CHECK(cudaGetLastError());
+}
+
+void KeepAliveHandle(yd_sched* s, int64_t now_ns, const uint64_t* ids, const int64_t* lens, size_t n,
+                     int64_t new_expires_in_ns, uint8_t* ok_out) {
+  if (n == 0) return;
+  YD_CUDA_CHECK(cudaSetDevice(s->device));
+  s->d_ok.ensure(n);
+  KeepAlive(s, now_ns, ids, lens, n, new_expires_in_ns, s->d_ok.as<uint8_t>());
+  YD_CUDA_CHECK(cudaMemcpyAsync(ok_out, s->d_ok.p, n, cudaMemcpyDeviceToHost, s->st));
+  YD_CUDA_CHECK(cudaStreamSynchronize(s->st));
+}
+}  // namespace
+}  // extern "C++"
+
 // KeepTaskAlive x n, cc:142-165.
 void yd_keep_task_alive(yd_sched* s, int64_t now_ns, const uint64_t* ids, size_t n, int64_t new_expires_in_ns,
                         uint8_t* ok_out) {
-  if (n == 0) return;
-  YD_CUDA_CHECK(cudaSetDevice(s->device));
-  s->d_ids.ensure(n * 8);
-  s->d_ok.ensure(n);
-  YD_CUDA_CHECK(cudaMemcpyAsync(s->d_ids.p, ids, n * 8, cudaMemcpyHostToDevice, s->st));
-  yd::k_keep_alive<<<(unsigned)((n + 255) / 256), 256, 0, s->st>>>(
-      s->d_ids.as<unsigned long long>(), (uint32_t)n, (long long)now_ns, (long long)new_expires_in_ns, s->ring(),
-      s->d_ok.as<uint8_t>());
-  YD_CUDA_CHECK(cudaGetLastError());
-  YD_CUDA_CHECK(cudaMemcpyAsync(ok_out, s->d_ok.p, n, cudaMemcpyDeviceToHost, s->st));
-  YD_CUDA_CHECK(cudaStreamSynchronize(s->st));
+  KeepAliveHandle(s, now_ns, ids, nullptr, n, new_expires_in_ns, ok_out);
+}
+
+// KeepTaskAlive x n, each with its own lease length.
+void yd_keep_tasks_alive(yd_sched* s, int64_t now_ns, const uint64_t* ids, const int64_t* new_expires_in_ns, size_t n,
+                         uint8_t* ok_out) {
+  KeepAliveHandle(s, now_ns, ids, new_expires_in_ns, n, 0, ok_out);
 }
 
 // FreeTask x n, cc:167-188.  Fire and forget: ordered on the solve stream.

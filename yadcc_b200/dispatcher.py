@@ -393,13 +393,24 @@ class TaskDispatcher:
     def keep_task_alive(self, task_id: int, new_expires_in: float, *, now: float = 0.0) -> bool:
         return bool(self.keep_tasks_alive([task_id], new_expires_in, now=now)[0])
 
-    def keep_tasks_alive(self, task_ids: Iterable[int], new_expires_in: float, *, now: float = 0.0) -> np.ndarray:
-        return self._keep_alive_with(self._lib.yd_keep_task_alive, task_ids, new_expires_in, now)
+    def keep_tasks_alive(self, task_ids: Iterable[int], new_expires_in: float | Sequence[float], *,
+                         now: float = 0.0) -> np.ndarray:
+        """KeepTaskAlive per id.  `new_expires_in` is one lease length for every id (yd_keep_task_alive) or one per id
+        (yd_keep_tasks_alive: the last occurrence of a repeated id sets its expiry)."""
+        each = None if np.ndim(new_expires_in) == 0 else self._optional_fn("yd_keep_tasks_alive")
+        return self._keep_alive_with(self._lib.yd_keep_task_alive, task_ids, new_expires_in, now, fn_each=each)
 
-    def _keep_alive_with(self, fn, task_ids, new_expires_in: float, now: float) -> np.ndarray:
+    def _keep_alive_with(self, fn, task_ids, new_expires_in, now: float, fn_each=None) -> np.ndarray:
         ids = np.ascontiguousarray(np.asarray(list(task_ids) if not isinstance(task_ids, np.ndarray) else task_ids, dtype=np.uint64))
         ok = np.zeros(ids.shape[0], dtype=np.uint8)
-        if fn(self._h, _ns(now), ids.ctypes.data, ids.shape[0], _ns(new_expires_in), ok.ctypes.data):
+        if np.ndim(new_expires_in) == 0:
+            rc = fn(self._h, _ns(now), ids.ctypes.data, ids.shape[0], _ns(new_expires_in), ok.ctypes.data)
+        else:
+            lens = np.ascontiguousarray([_ns(x) for x in new_expires_in], dtype=np.int64)
+            if lens.shape != ids.shape or fn_each is None:
+                raise ValueError("one lease length per id")
+            rc = fn_each(self._h, _ns(now), ids.ctypes.data, lens.ctypes.data, ids.shape[0], ok.ctypes.data)
+        if rc:
             raise RuntimeError("keep-alive refused")
         return ok.astype(bool)
 

@@ -92,29 +92,56 @@ class SchedulerService:
         except Exception:
             pass
 
-    def heartbeat(self, req: HeartbeatRequest, *, now: float = 0.0) -> HeartbeatResponse:
+    @staticmethod
+    def _heartbeat_struct(req: HeartbeatRequest, keep: list):
+        """The request struct and the response's expired-ids buffer; `keep` owns what they point to."""
         envs = [e.encode() for e in req.env_digests]
         env_arr = (C.c_char_p * max(len(envs), 1))(*envs)
         n = len(req.running_tasks)
         tasks = (_abi.yd_running_task * max(n, 1))()
-        keep = []
         for i, t in enumerate(req.running_tasks):
             loc, dig = t.servant_location.encode(), t.task_digest.encode()
             keep.append((loc, dig))
             tasks[i] = _abi.yd_running_task(t.servant_task_id, t.task_grant_id, loc, dig)
         expired = (C.c_uint64 * max(n, 1))()
+        strs = (req.token.encode(), req.location.encode(), req.remote_ip.encode())
+        keep.append((envs, env_arr, tasks, expired, strs))
         r = _abi.yd_heartbeat_request(
-            req.token.encode(), req.location.encode(), req.remote_ip.encode(), int(req.remote_is_ipv6),
+            strs[0], strs[1], strs[2], int(req.remote_is_ipv6),
             req.next_heartbeat_in_ms, req.version, req.num_processors, req.current_load, req.servant_priority,
             req.not_accepting_task_reason, req.capacity, len(envs), req.total_memory_in_bytes,
             req.memory_available_in_bytes, env_arr, tasks, n)
-        resp = _abi.yd_heartbeat_response()
-        resp.expired_tasks = expired
-        st = self._lib.yd_service_heartbeat(self._h, _ns(now), C.byref(r), C.byref(resp))
+        return r, expired
+
+    @staticmethod
+    def _heartbeat_answer(st: int, resp, expired) -> HeartbeatResponse:
         if st != STATUS_OK:
             return HeartbeatResponse(st, [], [])
         return HeartbeatResponse(st, [resp.acceptable_tokens[i].decode() for i in range(3)],
                                  [int(expired[i]) for i in range(resp.n_expired_tasks)])
+
+    def heartbeat(self, req: HeartbeatRequest, *, now: float = 0.0) -> HeartbeatResponse:
+        keep: list = []
+        r, expired = self._heartbeat_struct(req, keep)
+        resp = _abi.yd_heartbeat_response()
+        resp.expired_tasks = expired
+        st = self._lib.yd_service_heartbeat(self._h, _ns(now), C.byref(r), C.byref(resp))
+        return self._heartbeat_answer(st, resp, expired)
+
+    def heartbeats(self, reqs: Sequence[HeartbeatRequest], *, now: float = 0.0) -> list[HeartbeatResponse]:
+        """A run of Heartbeat RPCs in one call (yd_service_heartbeats): the answers of `heartbeat` on each in order."""
+        n = len(reqs)
+        keep: list = []
+        rq = (_abi.yd_heartbeat_request * max(n, 1))()
+        rs = (_abi.yd_heartbeat_response * max(n, 1))()
+        bufs = []
+        for i, req in enumerate(reqs):
+            rq[i], expired = self._heartbeat_struct(req, keep)
+            rs[i].expired_tasks = expired
+            bufs.append(expired)
+        st = (C.c_int * max(n, 1))()
+        self._lib.yd_service_heartbeats(self._h, _ns(now), rq, n, rs, st)
+        return [self._heartbeat_answer(st[i], rs[i], bufs[i]) for i in range(n)]
 
     def get_config(self, token: str, *, now: float = 0.0) -> tuple[int, str | None]:
         out = C.c_char_p()
@@ -145,6 +172,37 @@ class SchedulerService:
         ids = np.ascontiguousarray(np.asarray(task_grant_ids, dtype=np.uint64))
         return self._lib.yd_service_free_task(self._h, token.encode(), ids.ctypes.data, len(ids))
 
+    def keep_tasks_alive(self, requests, *, now: float = 0.0) -> list[tuple[int, np.ndarray]]:
+        """A run of KeepTaskAlive RPCs, [(token, task_grant_ids, next_keep_alive_in_ms)], in one call
+        (yd_service_keep_tasks_alive): the answers of `keep_task_alive` on each in order."""
+        n = len(requests)
+        rq = (_abi.yd_keep_task_alive_request * max(n, 1))()
+        keep = []
+        for i, (token, task_grant_ids, ms) in enumerate(requests):
+            ids = np.ascontiguousarray(np.asarray(task_grant_ids, dtype=np.uint64))
+            ok = np.zeros(max(len(ids), 1), dtype=np.uint8)
+            tok = token.encode()
+            keep.append((ids, ok, tok))
+            rq[i] = _abi.yd_keep_task_alive_request(tok, ms, ids.ctypes.data, len(ids), ok.ctypes.data)
+        st = (C.c_int * max(n, 1))()
+        self._lib.yd_service_keep_tasks_alive(self._h, _ns(now), rq, n, st)
+        return [(st[i], keep[i][1][:len(keep[i][0])].astype(bool)) for i in range(n)]
+
+    def free_tasks(self, requests) -> list[int]:
+        """A run of FreeTask RPCs, [(token, task_grant_ids)], in one call (yd_service_free_tasks): the statuses of
+        `free_task` on each in order."""
+        n = len(requests)
+        rq = (_abi.yd_free_task_request * max(n, 1))()
+        keep = []
+        for i, (token, task_grant_ids) in enumerate(requests):
+            ids = np.ascontiguousarray(np.asarray(task_grant_ids, dtype=np.uint64))
+            tok = token.encode()
+            keep.append((ids, tok))
+            rq[i] = _abi.yd_free_task_request(tok, ids.ctypes.data, len(ids))
+        st = (C.c_int * max(n, 1))()
+        self._lib.yd_service_free_tasks(self._h, rq, n, st)
+        return [st[i] for i in range(n)]
+
     def get_running_tasks(self) -> list[RunningTask]:
         n = self._lib.yd_service_get_running_tasks(self._h, None, 0)
         arr = (_abi.yd_running_task * max(n, 1))()
@@ -156,7 +214,7 @@ class SchedulerService:
     # -- FlareStd wire front end (include/ydwire.h) ---------------------------------
     def handle_frames(self, frames, *, now: float = 0.0, out_cap: int | None = None):
         """frames: [(bytes, remote_ip[, is_ipv6])], the first frame of each is handled, in order
-        (consecutive WaitForStartingTask frames as one batched solve).  Returns a list of
+        (consecutive Heartbeat, WaitForStartingTask, KeepTaskAlive or FreeTask frames as one batch).  Returns a list of
         (verdict, consumed, status, response_bytes)."""
         n = len(frames)
         ins = (_abi.yd_wire_in * max(n, 1))()

@@ -317,11 +317,13 @@ class RangeShardedDispatcher:
 
     # -- replicated calls (ydshard.h): every rank makes the call with the same arguments and gets the single scheduler's
     # answer.  Over gloo with the CPU libraries every replica holds every lease, so these are the local calls there.
-    def keep_tasks_alive(self, ids, new_expires_in: float, *, now: float = 0.0) -> np.ndarray:
-        """Replicated KeepTaskAlive: the holder of each lease renews it; every rank returns the same flags."""
+    def keep_tasks_alive(self, ids, new_expires_in, *, now: float = 0.0) -> np.ndarray:
+        """Replicated KeepTaskAlive: the holder of each lease renews it; every rank returns the same flags.
+        `new_expires_in` is one lease length, or one per id (yd_shard_keep_tasks_alive)."""
         if not self.native:
             return self.local.keep_tasks_alive(ids, new_expires_in, now=now)
-        return self.local._keep_alive_with(self.local._lib.yd_shard_keep_task_alive, ids, new_expires_in, now)
+        return self.local._keep_alive_with(self.local._lib.yd_shard_keep_task_alive, ids, new_expires_in, now,
+                                           fn_each=self.local._lib.yd_shard_keep_tasks_alive)
 
     def notify_servants_running_tasks(self, batch) -> list[list[int]]:
         """Replicated NotifyServantRunningTasks for [(location, tasks)]: an id is unknown iff no rank holds its lease."""

@@ -6,13 +6,15 @@
 #                      checkers/libydport_keys.so and oracle/_ref/libydref_keys.so: port and reference with the task keys)
 #   make fake_nccl  -> tests/fake_nccl/libnccl.so.2: the test-only NCCL stand-in that runs several ranks of the
 #                      range-sharded scheduler as threads of one process on one GPU (tests/test_shard_one_gpu.py)
+#   make primitives -> tests/kernels/libydprim.so: host wrappers that launch the product's device primitives on their own
+#                      (tests/test_device_primitives.py)
 NVCC ?= /usr/local/cuda/bin/nvcc
 ARCH = -gencode arch=compute_90a,code=sm_90a
 NVCCFLAGS = -O3 -std=c++17 -lineinfo $(ARCH) -Xcompiler -fPIC,-Wall,-Wno-unused-function -Iinclude -Iyadcc_b200/csrc
 CSRC = yadcc_b200/csrc
 LIB = yadcc_b200/libydsched.so
 
-all: cuda oracle fake_nccl
+all: cuda oracle fake_nccl primitives
 
 cuda: $(LIB)
 
@@ -35,8 +37,14 @@ fake_nccl: $(FAKE_NCCL)
 $(FAKE_NCCL): tests/fake_nccl/fake_nccl.cc
 	$(CXX) -std=c++17 -O2 -fPIC -Wall -shared -Wl,-soname,libnccl.so.2 -o $@ $< -ldl -pthread
 
+PRIM = tests/kernels/libydprim.so
+primitives: $(PRIM)
+
+$(PRIM): tests/kernels/primitives.cu $(CSRC)/radix.cuh $(CSRC)/filter.cuh $(CSRC)/state.cuh $(CSRC)/common.cuh include/ydsched.h include/ydstate.h
+	$(NVCC) $(NVCCFLAGS) -shared -o $@ tests/kernels/primitives.cu
+
 clean:
-	rm -f $(LIB) $(FAKE_NCCL) checkers/libydport_state.so checkers/libydport_keys.so oracle/_ref/libydref_keys.so
+	rm -f $(LIB) $(FAKE_NCCL) $(PRIM) checkers/libydport_state.so checkers/libydport_keys.so oracle/_ref/libydref_keys.so
 	$(MAKE) -C oracle clean
 
-.PHONY: all cuda oracle fake_nccl clean
+.PHONY: all cuda oracle fake_nccl primitives clean

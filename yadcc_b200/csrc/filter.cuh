@@ -13,6 +13,7 @@
 //   k_keep_scatter  survivors -> the solver's queue, FIFO order kept (16-byte requests are unpacked on the way)
 #pragma once
 #include "common.cuh"
+#include "radix.cuh"  // k_scan_u32
 
 namespace yd {
 
@@ -68,6 +69,23 @@ __global__ void __launch_bounds__(1024) k_keep_scatter(const Req* __restrict__ i
   for (uint32_t w = 0; w < warp; ++w) before += warp_cnt[w];
   before += __popc(bal & ((1u << lane) - 1));
   keep_put(in + q, out + before);
+}
+
+// The compaction's first two launches on `st`, for a queue of n >= 1 requests (callers answer an empty queue without
+// launching): the verdicts, and in tile_off (ceil(n / 1024) + 1 words) the survivors' offsets per tile of 1024 with
+// their total behind them.
+inline void keep_count_scan(const uint8_t* bloom_hit, const uint4* rt_hit, uint32_t n, uint8_t* verdict, uint32_t* tile_off,
+                            cudaStream_t st) {
+  const uint32_t nt = (n + 1023) / 1024;
+  k_keep_count<<<nt, 1024, 0, st>>>(bloom_hit, rt_hit, n, verdict, tile_off);
+  k_scan_u32<<<1, 1024, 0, st>>>(tile_off, nt + 1, nullptr, 0, nullptr, 0);
+}
+
+// Its last launch: the survivors of `in` (n requests, verdicts and tile offsets from keep_count_scan) -> out, in order.
+template <class Req>
+inline void keep_scatter(const Req* in, const uint8_t* verdict, const uint32_t* tile_off, uint32_t n, yd_task_req* out,
+                         cudaStream_t st) {
+  k_keep_scatter<<<(n + 1023) / 1024, 1024, 0, st>>>(in, verdict, tile_off, n, out);
 }
 
 }  // namespace yd

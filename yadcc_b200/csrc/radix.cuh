@@ -343,4 +343,28 @@ __global__ void __launch_bounds__(kRsThreads) k_rs_pass(const KeyT* __restrict__
   }
 }
 
+// The whole sort on `st`: stable by bits [first_bit, first_bit + 7 * passes) of the keys, passes = (last_bit - first_bit)
+// / 7 + 1, payloads starting as the keys' indices.  n = *n_ptr (known on the device only), nb >= ceil(n / kRsTile) tiles.
+// The digit histograms of all passes in one read, then one kernel per pass, ping-ponging between buffers 0 and 1 of
+// keys_out / vals_out so that the LAST pass writes buffer 0 (captured graphs keep its address); keys_in is only read.
+// zbase: rs_pass_words(nb) words per pass, zeroed by the caller.  Returns the number of kernels launched.
+template <typename KeyT>
+inline uint32_t rs_sort(const KeyT* keys_in, const unsigned long long* n_ptr, uint32_t nb, int first_bit, int last_bit,
+                        uint32_t* zbase, KeyT* const keys_out[2], uint32_t* const vals_out[2], cudaStream_t st) {
+  const size_t stride = rs_pass_words(nb);
+  const int passes = (last_bit - first_bit) / kRsBits + 1;
+  const KeyT* kin = keys_in;
+  const uint32_t* vin = nullptr;
+  int cur = (passes - 1) & 1;
+  k_rs_ghist<KeyT><<<nb, kRsThreads, 0, st>>>(kin, n_ptr, first_bit, passes, nb, zbase);
+  for (int pass = 0; pass < passes; ++pass) {
+    k_rs_pass<KeyT><<<nb, kRsThreads, 0, st>>>(kin, vin, n_ptr, first_bit + pass * kRsBits, nb,
+                                               rs_pass_scratch(zbase + pass * stride, nb), keys_out[cur], vals_out[cur]);
+    kin = keys_out[cur];
+    vin = vals_out[cur];
+    cur ^= 1;
+  }
+  return 1 + passes;
+}
+
 }  // namespace yd

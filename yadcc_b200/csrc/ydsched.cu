@@ -957,29 +957,11 @@ uint32_t LaunchRowscan(yd_sched* s) {
 
 template <typename KeyT>
 uint32_t LaunchSort(yd_sched* s, int first_bit, int last_bit) {
-  cudaStream_t st = s->st;
-  const uint32_t nb = s->sort_nb;
-  const unsigned long long* n_ptr = &s->d_counters.as<Counters>()->slots;
-  uint32_t* zbase = reinterpret_cast<uint32_t*>(static_cast<char*>(s->d_zero.p) + s->z_hist_off[0]);
-  const size_t stride = yd::rs_pass_words(nb);
-  const int passes = (last_bit - first_bit) / yd::kRsBits + 1;
-  const KeyT* kin = s->d_codes.as<KeyT>();
-  const uint32_t* vin = nullptr;
-  int cur = (passes - 1) & 1;  // ping-pong so that the LAST pass writes buffer 0 (captured graphs keep its address)
-  // digit histograms of all passes in one read, then one kernel per pass
-  yd::k_rs_ghist<KeyT><<<nb, yd::kRsThreads, 0, st>>>(kin, n_ptr, first_bit, passes, nb, zbase);
-  uint32_t launches = 1;
-  for (int pass = 0; pass < passes; ++pass) {
-    KeyT* kout = s->d_sort_k[cur].as<KeyT>();
-    uint32_t* vout = s->d_sort_v[cur].as<uint32_t>();
-    yd::k_rs_pass<KeyT><<<nb, yd::kRsThreads, 0, st>>>(kin, vin, n_ptr, first_bit + pass * yd::kRsBits, nb,
-                                                       yd::rs_pass_scratch(zbase + pass * stride, nb), kout, vout);
-    launches += 1;
-    kin = kout;
-    vin = vout;
-    cur ^= 1;
-  }
-  return launches;
+  KeyT* const keys[2] = {s->d_sort_k[0].as<KeyT>(), s->d_sort_k[1].as<KeyT>()};
+  uint32_t* const vals[2] = {s->d_sort_v[0].as<uint32_t>(), s->d_sort_v[1].as<uint32_t>()};
+  return yd::rs_sort<KeyT>(s->d_codes.as<KeyT>(), &s->d_counters.as<Counters>()->slots, s->sort_nb, first_bit, last_bit,
+                           reinterpret_cast<uint32_t*>(static_cast<char*>(s->d_zero.p) + s->z_hist_off[0]), keys, vals,
+                           s->st);
 }
 
 // Merge-solver chunk: more, shorter chunks pay while the request-side passes are short (measured on an H100 SXM, 700 W:
@@ -2419,13 +2401,12 @@ struct FilterKeys {
 
 // The compaction: the offered requests of d_freqs (24-byte records, or with `req16` 16-byte ones) -> the solver's queue.
 static void KeepScatter(yd_sched* s, uint32_t N, bool req16) {
-  const uint32_t nt = (N + 1023) / 1024;
   if (req16) {
-    yd::k_keep_scatter<<<nt, 1024, 0, s->st>>>(s->d_freqs.as<yd_task_req16>(), s->d_fverdict.as<uint8_t>(),
-                                               s->d_ftile.as<uint32_t>(), N, s->d_reqs.as<yd_task_req>());
+    yd::keep_scatter(s->d_freqs.as<yd_task_req16>(), s->d_fverdict.as<uint8_t>(), s->d_ftile.as<uint32_t>(), N,
+                     s->d_reqs.as<yd_task_req>(), s->st);
   } else {
-    yd::k_keep_scatter<<<nt, 1024, 0, s->st>>>(s->d_freqs.as<yd_task_req>(), s->d_fverdict.as<uint8_t>(),
-                                               s->d_ftile.as<uint32_t>(), N, s->d_reqs.as<yd_task_req>());
+    yd::keep_scatter(s->d_freqs.as<yd_task_req>(), s->d_fverdict.as<uint8_t>(), s->d_ftile.as<uint32_t>(), N,
+                     s->d_reqs.as<yd_task_req>(), s->st);
   }
 }
 
@@ -2464,10 +2445,8 @@ static size_t FilterStages(yd_sched* s, int64_t now_ns, uint32_t N, const Filter
                                                      N, s->d_rt_ids.as<unsigned long long>(), s->d_rt_out.as<uint4>());
     }
   }
-  yd::k_keep_count<<<nt, 1024, 0, st>>>(k.bloom ? s->d_bloom_out.as<uint8_t>() : nullptr,
-                                        k.dedupe ? s->d_rt_out.as<uint4>() : nullptr, N, s->d_fverdict.as<uint8_t>(),
-                                        s->d_ftile.as<uint32_t>());
-  yd::k_scan_u32<<<1, 1024, 0, st>>>(s->d_ftile.as<uint32_t>(), nt + 1, nullptr, 0, nullptr, 0);
+  yd::keep_count_scan(k.bloom ? s->d_bloom_out.as<uint8_t>() : nullptr, k.dedupe ? s->d_rt_out.as<uint4>() : nullptr, N,
+                      s->d_fverdict.as<uint8_t>(), s->d_ftile.as<uint32_t>(), st);
   KeepScatter(s, N, req16);
   YD_CUDA_CHECK(cudaGetLastError());
   YD_CUDA_CHECK(cudaEventRecord(s->ev_f[1], st));

@@ -377,7 +377,7 @@ struct yd_sched {
   yd_solve_stats stats{};
   bool have_stats = false;
   int stats_times_pending = 0;  // 1: events of an eager general solve, 2: of a graphed or solo one, not yet turned into milliseconds
-  size_t static_bound_cache = 0;  // StaticSlotBound() of the current facts
+  size_t static_bound_cache = 0;  // the sum over the servants of min(nproc, max_tasks) + 1 (SyncFacts): the kept slot table's bound
 
   yd::ServantArrays arrays() const {
     return yd::ServantArrays{d_nproc.as<uint32_t>(), d_load.as<uint32_t>(), d_maxt.as<uint32_t>(),
@@ -1348,8 +1348,31 @@ uint64_t NextPow2(uint64_t v, uint64_t lo) {
   return r;
 }
 
+// What turns the packed grants of the next batch into task ids (yd_packed_ids): its first task id and the stride.
+yd_packed_ids BatchIds(const yd_sched* s) { return yd_packed_ids{s->next_id * s->id_stride + s->id_offset, s->id_stride}; }
+
+// One call decides at most 2^30 requests (packed grant ordinals have 30 bits).
+void CheckBatchSize(size_t n) {
+  if (n > 0x40000000ull) { fprintf(stderr, "ydsched: batch too large\n"); abort(); }
+}
+
+// yd_last_solve_stats reports zeros from here on, until the caller fills fields in.
+void ResetStats(yd_sched* s) { s->stats = yd_solve_stats{}; s->stats_times_pending = 0; s->have_stats = true; }
+
+// n requests as 24-byte records: copied from `reqs`, or unpacked from `reqs16`.
+void CopyRequests(const yd_task_req* reqs, const yd_task_req16* reqs16, size_t n, yd_task_req* r) {
+  if (reqs) memcpy(r, reqs, n * sizeof(yd_task_req));
+  else for (size_t i = 0; i != n; ++i) r[i] = yd_unpack_req(reqs16[i]);
+}
+
+// n grants to the caller: 16-byte records to `out`, or packed with the batch's `ids` to `out8`.
+void WriteGrants(yd_grant* out, yd_grant8* out8, const yd_packed_ids& ids, const yd_grant* g, size_t n) {
+  if (out8) for (size_t i = 0; i != n; ++i) out8[i] = yd_pack_grant(g[i], ids);
+  else if (n) memcpy(out, g, n * sizeof(yd_grant));
+}
+
 // Everything between the request upload and the grant download, for size class (Nb, slot_b), of a general (not solo)
-// solve: the sequence that is captured into a CUDA graph.  (A solo solve is one kernel: WaitImpl launches it.)
+// solve: the sequence that is captured into a CUDA graph.  (A solo solve is one kernel: LaunchSolo launches it.)
 // packed bit 0: the upload is 16-byte records in d_reqs16; bit 1: the download is 8-byte grants from d_out8.
 // `copied`: this call copied the requests on the copy stream (WaitUpload).
 uint32_t EnqueueSolve(yd_sched* s, uint32_t Nb, const SolveGeometry& g, const SolvePlan& plan, bool record_events,
@@ -1429,7 +1452,7 @@ uint32_t EnqueueSolve(yd_sched* s, uint32_t Nb, const SolveGeometry& g, const So
 // Queue staging: a front end can move the pending queue into HBM while RPCs are still
 // arriving and start the solve when the batch closes.
 void yd_stage_requests(yd_sched* s, const yd_task_req* reqs, size_t n) {
-  if (n > 0x40000000ull) { fprintf(stderr, "ydsched: batch too large\n"); abort(); }
+  CheckBatchSize(n);
   YD_CUDA_CHECK(cudaSetDevice(s->device));
   s->staged_n = 0;
   if (n == 0) return;
@@ -1447,18 +1470,264 @@ void yd_wait_for_staged_tasks(yd_sched* s, int64_t now_ns, size_t n, yd_grant* o
 
 extern "C++" {
 namespace {
+// YDSCHED_HOST_PROF: host-side timestamps of a solve (microseconds; 0 when off), printed at its end.
+struct HostProf {
+  bool on;
+  double t[8] = {};
+  void Stamp(int i) { if (on) t[i] = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
+  void Print() {
+    if (!on) return;
+    Stamp(7);
+    fprintf(stderr, "ydsched: host us: prep %.1f (attrs+variant %.1f) upload+prep %.1f launch %.1f d2h-enqueue %.1f sync-wait %.1f stats %.1f total %.1f\n",
+            t[1] - t[0], t[2] - t[1], t[3] - t[2], t[4] - t[3], t[5] - t[4], t[6] - t[5], t[7] - t[6], t[7] - t[0]);
+  }
+};
+
+// A handful of requests on the default solver: one launch, arguments in, pinned memory out (tiny.cuh).  Returns whether
+// it decided the batch.
+bool TinySolve(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_task_req16* reqs16, uint32_t N, yd_grant* out,
+               yd_grant8* out8, const yd_packed_ids& ids) {
+  if ((!reqs && !reqs16) || N > yd::kTinyMax || s->solver_pref != 0 || !s->tiny_ok || s->sv.empty() || !s->n_comps) return false;
+  s->h_small.ensure(256);
+  yd::TinyArgs ta{};
+  CopyRequests(reqs, reqs16, N, ta.reqs);
+  ta.n = N; ta.now_ns = now_ns; ta.t = MakeTopo(s); ta.sv = s->arrays(); ta.ring = s->ring();
+  ta.out = s->h_small.as<yd_grant>();
+  ta.granted_out = reinterpret_cast<unsigned long long*>(s->h_small.as<char>() + yd::kTinyMax * sizeof(yd_grant));
+  ta.counters = s->d_counters.as<Counters>();
+  YD_CUDA_CHECK(cudaEventRecord(s->ev[0], s->st));
+  yd::k_solve_tiny<<<1, 1024, 0, s->st>>>(ta);
+  YD_CUDA_CHECK(cudaGetLastError());
+  YD_CUDA_CHECK(cudaEventRecord(s->ev[5], s->st));
+  YD_CUDA_CHECK(cudaStreamSynchronize(s->st));
+  WriteGrants(out, out8, ids, ta.out, N);
+  const unsigned long long granted = *ta.granted_out;
+  s->next_id += granted;
+  s->staged_n = 0;
+  float ms = 0;
+  cudaEventElapsedTime(&ms, s->ev[0], s->ev[5]);
+  ResetStats(s);
+  yd_solve_stats& stt = s->stats;
+  stt.total_ms = stt.solve_ms = ms;
+  stt.decisions = N; stt.granted = granted; stt.kernel_launches = 1; stt.solver = 3;
+  stt.h2d_bytes = 0;  // the requests are kernel arguments
+  stt.d2h_bytes = size_t(N) * sizeof(yd_grant) + 8;  // written by the kernel into pinned host memory
+  if (s->debug_env) {
+    fprintf(stderr, "ydsched: solve n %u tiny 1 solver 3 spec 0 ring_cap %llu ring_lo %llu solve_ms %.3f\n", N,
+            (unsigned long long)s->ring_cap, (unsigned long long)s->lo, ms);
+  }
+  return true;
+}
+
+// The device address of a page-locked caller array (yd_alloc_host), or null: pageable, or not 16-byte aligned.
+void* MappedAddress(const void* p) {
+  if (!p || (reinterpret_cast<uintptr_t>(p) & 15u)) return nullptr;
+  cudaPointerAttributes at{};
+  if (cudaPointerGetAttributes(&at, p) != cudaSuccess) { cudaGetLastError(); return nullptr; }
+  return at.type == cudaMemoryTypeHost ? at.devicePointer : nullptr;
+}
+
+// The variant of an attempt (SoloTables::Choose); `now` is set to the kept-table signature a solo variant runs on.
+SolveVariant ChooseVariant(yd_sched* s, uint32_t Nb, const SolveGeometry& geo, uint32_t solver, bool want_static, KeptSig& now) {
+  const uint32_t S = (uint32_t)s->sv.size();
+  // The fused front kernel takes batches in the latency-bound regime whose (class, tile) count matrices one block
+  // scans in a few rounds; it needs the kept slot order.  Solo = it also writes the grants (no coupled component
+  // had requests last time; if one has now, the kernel raises flag 4 and the batch is replayed with kFused).
+  const bool fused = s->fused_cfg && s->fused_grid && s->solver_pref == 0 && solver == 2 && want_static && S &&
+                     s->n_comps && Nb <= s->fused_max_nb && size_t(s->cls_bound) * geo.n_rtiles <= 32768 &&
+                     size_t(s->cls_bound) * geo.n_ltiles <= 32768;
+  if (fused && s->solo.hint) {
+    now = KeptSig{CleanSig{g_buf_generation, s->z_cls_off, s->z_bytes, s->res_words, s->d_zero.p, s->d_res.p},
+                  s->topo_gen, s->cls_bound};
+  }
+  // speculative (fused.cuh): every block holds at most two request tiles (their classes and ranks stay in
+  // registers), the lists' offsets fit in shared memory, and registry positions fit the member words below the slot's
+  // index in its tile (classes.cuh: kMemberSlotShift)
+  const bool spec_ok = FusedLoffWords(s, geo) != 0 && geo.n_rtiles <= 2 * s->fused_grid && S <= yd::kMemberPosMask;
+  return s->solo.Choose(fused, now, spec_ok);
+}
+
+// A solo solve: ONE kernel whose per-call scalars are kernel parameters, launched directly, as a graph would add a
+// parameter patch and a graph launch to the call.  Its arguments are built before the events, which bracket what the
+// solve enqueues on `st`; the kernel leaves grant count and flags in the mapped host record.  Returns the launches.
+uint32_t LaunchSolo(yd_sched* s, uint32_t Nb, const SolveGeometry& geo, const SolvePlan& plan, bool copied, uint32_t packed,
+                    HostProf& hp) {
+  cudaStream_t st = s->st;
+  const yd::FusedArgs a = MakeFusedArgs(s, Nb, geo, plan, false, packed & 1u, packed & 2u);
+  hp.Stamp(3);
+  YD_CUDA_CHECK(cudaEventRecord(s->ev[1], st));
+  if (plan.variant == kSolo) {
+    // the solo kernel keeps the verdicts in registers: only the class-table keys behind res[] are initialised --
+    // and not even those when the previous solo solve left the scratch clean (kSoloClean, kSoloSpec)
+    YD_CUDA_CHECK(cudaMemsetAsync(s->d_res.as<uint32_t>() + s->res_words, 0xFF, yd::kClsTableSize * 8, st));
+    YD_CUDA_CHECK(cudaMemsetAsync(static_cast<char*>(s->d_zero.p) + s->z_cls_off, 0, s->z_bytes - s->z_cls_off, st));
+  }
+  WaitUpload(s, st, copied, false);
+  LaunchFusedKernel(s, a);
+  YD_CUDA_CHECK(cudaEventRecord(s->ev[4], st));
+  hp.Stamp(4);
+  YD_CUDA_CHECK(cudaGetLastError());
+  return 1;
+}
+
+// A general solve through the graph of its size class (EnqueueSolve, captured on first use).  Returns its launches.
+uint32_t LaunchGraphed(yd_sched* s, uint32_t Nb, size_t slot_b, const SolveGeometry& geo, const SolvePlan& plan, bool copied,
+                       uint32_t packed, HostProf& hp) {
+  cudaStream_t st = s->st;
+  yd_sched::GraphKey key;
+  key.Nb = Nb; key.S = (uint32_t)s->sv.size(); key.n_comps = s->n_comps; key.max_comp = s->max_comp_servants;
+  key.cls_bound = s->cls_bound; key.solver = plan.solver; key.wide = s->wide; key.slot_b = slot_b;
+  key.gen = g_buf_generation; key.topo_gen = s->topo_gen; key.ring_cap = s->ring_cap;
+  key.merge_rounds = plan.merge_rounds; key.force_stream = plan.force_stream;
+  key.order_static = (plan.solver == 2 && s->order_static) ? 1u : 0u;
+  key.variant = plan.variant; key.packed = packed;
+  yd_sched::GraphEntry* hit = nullptr;
+  for (auto& g : s->graphs) if (g.key == key) { hit = &g; break; }
+  if (!hit) {
+    cudaGraph_t graph = nullptr;
+    YD_CUDA_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+    uint32_t l = EnqueueSolve(s, Nb, geo, plan, false, copied, true, packed);
+    YD_CUDA_CHECK(cudaStreamEndCapture(st, &graph));
+    cudaGraphExec_t exec = nullptr;
+    YD_CUDA_CHECK(cudaGraphInstantiate(&exec, graph, 0));
+    YD_CUDA_CHECK(cudaGraphDestroy(graph));
+    if (s->graphs.size() >= 16) {  // drop the oldest size class
+      cudaGraphExecDestroy(s->graphs.front().exec);
+      s->graphs.erase(s->graphs.begin());
+    }
+    s->graphs.push_back(yd_sched::GraphEntry{key, exec, l});
+    hit = &s->graphs.back();
+  }
+  hp.Stamp(3);
+  YD_CUDA_CHECK(cudaEventRecord(s->ev[1], st));
+  YD_CUDA_CHECK(cudaGraphLaunch(hit->exec, st));
+  YD_CUDA_CHECK(cudaEventRecord(s->ev[4], st));
+  hp.Stamp(4);
+  return hit->launches;
+}
+
+// YDSCHED_FUSED_PROF: the fused kernel's phase stamps after an attempt of `variant` on a batch of N.
+void PrintFusedProfile(yd_sched* s, SolveVariant variant, uint32_t N) {
+  if (variant == kSoloSpec) {
+    unsigned long long t[9];
+    YD_CUDA_CHECK(cudaMemcpy(t, s->d_fused_prof.p, sizeof t, cudaMemcpyDeviceToHost));
+    if (s->h_meta.as<uint32_t>()[1] == yd::kFlagSpecMiss) {  // (no phase B)
+      fprintf(stderr, "ydsched: fused variant 4 (speculative) n %u ns: A %llu barrier %llu missed\n", N, t[1] - t[0], t[2] - t[1]);
+    } else {
+      fprintf(stderr, "ydsched: fused variant 4 (speculative) n %u ns: A %llu barrier %llu B %llu total %llu (+tail %lld)\n", N,
+              t[1] - t[0], t[2] - t[1], t[7] - t[2], t[7] - t[0], (long long)(t[8] - t[7]));
+    }
+    // every block's stamps (fused.cuh: kProfBlockWords), for tools/dev/phase_prof.py
+    const uint32_t G = s->fused_grid;
+    std::vector<unsigned long long> b(size_t(G) * yd::kProfBlockWords);
+    YD_CUDA_CHECK(cudaMemcpy(b.data(), s->d_fused_prof.as<unsigned long long>() + yd::kProfHead, b.size() * 8,
+                             cudaMemcpyDeviceToHost));
+    std::string line = "ydsched: fused blocks " + std::to_string(G) + " last_end " + std::to_string(t[8]) + " stamps";
+    for (unsigned long long v : b) line += " " + std::to_string(v);
+    fprintf(stderr, "%s\n", line.c_str());
+  } else if (variant != kPipeline) {
+    unsigned long long t[9];
+    YD_CUDA_CHECK(cudaMemcpy(t, s->d_fused_prof.p, sizeof t, cudaMemcpyDeviceToHost));
+    fprintf(stderr, "ydsched: fused variant %u n %u ns: P1 %llu E1 %llu P3 %llu E2 %llu P5 %llu B3 %llu P6 %llu total %llu (+report/clean %lld)\n",
+            (unsigned)variant, N, t[1] - t[0], t[2] - t[1], t[3] - t[2], t[4] - t[3], t[5] - t[4], t[6] - t[5], t[7] - t[6],
+            t[7] - t[0], (long long)(t[8] - t[7]));
+  }
+}
+
+// A call's stand-downs so far; `spec`: the speculative variant 0 not tried, 1 decided the batch, 2 missed (replayed).
+struct StandDowns { int grow = 0, merge = 0; uint32_t spec = 0; };
+enum AttemptEnd { kDecided, kAgain, kHalves };
+
+// After an attempt, by its flag (meta[1]).  A slot-stream attempt with a flag decided nothing (the stream solver and
+// the final kernels all stood down): `plan` is set up for the next attempt, or the batch is decided in halves.
+AttemptEnd StandDown(yd_sched* s, SolvePlan& plan, StandDowns& d) {
+  const uint32_t* meta = s->h_meta.as<uint32_t>();
+  const uint32_t flag = meta[1];
+  if (plan.solver != 2 || s->sv.empty() || !s->n_comps || flag == 0) {
+    if (plan.variant == kSoloSpec) d.spec = 1;
+    return kDecided;
+  }
+  if (flag == yd::kFlagSpecMiss) {
+    // the kept class table could not decide the batch: replay without speculation (which builds the table again)
+    d.spec = 2;
+  } else if (flag == 4) {
+    // the solo kernel met a component it cannot decide: the general sequence, now and next time (SoloTables::Take)
+  } else if (flag == 2 && d.grow++ < 3 && GrowClassBound(s, meta)) {
+    // more lists than provisioned: go again with the grown class bound
+  } else if (flag == 3 && d.merge < 2) {
+    // the merge solver's boundary states had not settled after the rounds in the graph: more
+    // rounds first, then the sequential solver for everything it would have decided
+    if (d.merge == 0) plan.MoreMergeRounds(s->merge_max_chunks);
+    else plan.force_stream = 2;
+    ++d.merge;
+  } else if (s->max_comp_servants > kRowscanMaxComponent) {
+    return kHalves;
+  } else {
+    plan.solver = 1;
+  }
+  return kAgain;
+}
+
+// More classes than the class table holds AND a component beyond the row-scan solver's reach.  n sequential decisions
+// are the first half's followed by the second half's: decide the batch as two consecutive halves (each with half the
+// requests, hence -- eventually -- few enough classes).  The stats are the second half's, with decisions = N.
+void SolveInHalves(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_task_req16* reqs16, uint32_t N,
+                   yd_grant* out, yd_grant8* out8, const yd_packed_ids& ids) {
+  if (N < 2) { fprintf(stderr, "ydsched: class table overflow on a single request\n"); abort(); }
+  std::vector<yd_task_req> r(N);
+  if (reqs || reqs16) CopyRequests(reqs, reqs16, N, r.data());
+  else YD_CUDA_CHECK(cudaMemcpy(r.data(), s->d_reqs.p, size_t(N) * sizeof(yd_task_req), cudaMemcpyDeviceToHost));
+  std::vector<yd_grant> g(N);
+  const uint32_t h = N / 2;
+  yd_wait_for_starting_new_tasks(s, now_ns, r.data(), h, g.data());
+  yd_wait_for_starting_new_tasks(s, now_ns, r.data() + h, N - h, g.data() + h);
+  WriteGrants(out, out8, ids, g.data(), N);
+  s->stats.decisions = N;
+}
+
+// The stats of a decided batch (of the last attempt).  The event arithmetic costs a driver call apiece: done when
+// yd_last_solve_stats asks, the events stay valid until the next solve.
+void RecordSolveStats(yd_sched* s, uint32_t N, uint32_t launches, const SolvePlan& plan, const yd_task_req* reqs,
+                      const yd_task_req16* reqs16, const yd_grant8* out8) {
+  ResetStats(s);
+  yd_solve_stats& stt = s->stats;
+  s->stats_times_pending = (s->use_graphs || IsSolo(plan.variant)) ? 2 : 1;  // (graphed or solo: one device interval)
+  stt.decisions = N; stt.granted = s->h_counters.as<Counters>()->granted; stt.kernel_launches = launches; stt.solver = plan.solver;
+  stt.h2d_bytes = (reqs ? size_t(N) * sizeof(yd_task_req) : reqs16 ? size_t(N) * sizeof(yd_task_req16) : 0) + sizeof(yd::DynParams);
+  stt.d2h_bytes = size_t(N) * (out8 ? sizeof(yd_grant8) : sizeof(yd_grant)) + sizeof(Counters) + 32;
+}
+
+// YDSCHED_DEBUG: which path the solve took (the last attempt, after any stand-down): `final` 0 = the solo kernel wrote
+// the grants, 1 = k_final_fused, 3 = k_final_count / k_final_scan / k_final_write; `spec` over all attempts; the lease
+// ring (`ring_lo` = the first live id) as the solve found it
+void PrintSolveLine(yd_sched* s, uint32_t N, uint32_t Nb, size_t slot_b, const SolvePlan& plan, uint32_t spec) {
+  const Counters* c = s->h_counters.as<Counters>();
+  const uint32_t nb = (Nb + 1023) / 1024;
+  const bool have_work = !s->sv.empty() && s->n_comps;
+  const uint32_t solver = plan.solver;
+  const bool solo = IsSolo(plan.variant), graphed = !solo && s->use_graphs;
+  const uint32_t final_path = (solo && have_work && solver == 2) ? 0u : (solver == 2 && have_work && nb <= 2048) ? 1u : 3u;
+  const auto back = solver == 2 && have_work && !solo ? MergeBack(s) : std::pair<uint32_t, uint32_t>{0, 0};
+  fprintf(stderr, "ydsched: solve n %u tiny 0 variant %u order_static %d wide %d Nb %u slot_b %zu cls_bound %u final %u "
+          "emask %d max_comp %zu solver %u graph %d merge_rounds %llu merge_chunks %llu walks %llu windows %llu "
+          "merge_back %u merge_back_n %u spec %u ring_cap %llu ring_lo %llu solve_ms %.3f\n",
+          N, (unsigned)plan.variant, (int)(solver == 2 && s->order_static), (int)s->wide, Nb, slot_b, s->cls_bound, final_path,
+          (int)s->emask_ok, (size_t)s->max_comp_servants, solver, (int)graphed, c->pad[0], c->pad[1], c->pad[2],
+          c->pad[3], back.first, back.second, spec, (unsigned long long)s->ring_cap, (unsigned long long)s->lo, s->stats.solve_ms);
+}
+
 // The solve behind yd_wait_for_starting_new_tasks and its packed twin.  Requests: `reqs` (24-byte records), or `reqs16`
 // (16-byte records), or neither = the first n staged requests (yd_stage_requests) are already in HBM.  Grants: `out`
-// (16-byte records) or `out8` (8-byte records, ids = ids_out->first_task_id + ordinal * stride).
+// (16-byte records) or `out8` (8-byte records, ids = first_task_id + ordinal * stride of BatchIds, also to ids_out).
 void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_task_req16* reqs16, size_t n, yd_grant* out,
               yd_grant8* out8, yd_packed_ids* ids_out) {
-  if (ids_out) { ids_out->first_task_id = s->next_id * s->id_stride + s->id_offset; ids_out->stride = s->id_stride; }
+  const yd_packed_ids ids = BatchIds(s);
+  if (ids_out) *ids_out = ids;
   if (n == 0) return;
-  double hp[8] = {};
-  auto hp_now = [&]() { return s->host_prof ? std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now().time_since_epoch()).count() : 0.0; };
-  hp[0] = hp_now();
+  HostProf hp{s->host_prof};
+  hp.Stamp(0);
   if (!reqs && !reqs16 && n > s->staged_n) { fprintf(stderr, "ydsched: NULL request array and nothing staged\n"); abort(); }
-  if (n > 0x40000000ull) { fprintf(stderr, "ydsched: batch too large\n"); abort(); }
+  CheckBatchSize(n);
   YD_CUDA_CHECK(cudaSetDevice(s->device));
   cudaStream_t st = s->st;
   const uint32_t N = (uint32_t)n;
@@ -1468,56 +1737,14 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
   s->SyncFacts();
   s->SyncTopology();
   s->EnsureRing(N);
-
-  // ---- a handful of requests: one launch, arguments in, pinned memory out (tiny.cuh) ------------------------------
-  if ((reqs || reqs16) && N <= yd::kTinyMax && s->solver_pref == 0 && s->tiny_ok && S && s->n_comps) {
-    s->h_small.ensure(256);
-    yd::TinyArgs ta{};
-    if (reqs) memcpy(ta.reqs, reqs, size_t(N) * sizeof(yd_task_req));
-    else for (uint32_t i = 0; i != N; ++i) ta.reqs[i] = yd_unpack_req(reqs16[i]);
-    ta.n = N;
-    ta.now_ns = now_ns;
-    ta.t = MakeTopo(s);
-    ta.sv = s->arrays();
-    ta.ring = s->ring();
-    ta.out = s->h_small.as<yd_grant>();
-    ta.granted_out = reinterpret_cast<unsigned long long*>(s->h_small.as<char>() + yd::kTinyMax * sizeof(yd_grant));
-    ta.counters = s->d_counters.as<Counters>();
-    YD_CUDA_CHECK(cudaEventRecord(s->ev[0], st));
-    yd::k_solve_tiny<<<1, 1024, 0, st>>>(ta);
-    YD_CUDA_CHECK(cudaGetLastError());
-    YD_CUDA_CHECK(cudaEventRecord(s->ev[5], st));
-    YD_CUDA_CHECK(cudaStreamSynchronize(st));
-    if (out) memcpy(out, ta.out, size_t(N) * sizeof(yd_grant));
-    else for (uint32_t i = 0; i != N; ++i) out8[i] = yd_pack_grant(ta.out[i], *ids_out);
-    const unsigned long long granted = *ta.granted_out;
-    s->next_id += granted;
-    s->staged_n = 0;
-    float ms = 0;
-    cudaEventElapsedTime(&ms, s->ev[0], s->ev[5]);
-    s->stats = yd_solve_stats{};
-    s->stats_times_pending = 0;
-    s->stats.total_ms = s->stats.solve_ms = ms;
-    s->stats.decisions = N;
-    s->stats.granted = granted;
-    s->stats.kernel_launches = 1;
-    s->stats.solver = 3;
-    s->stats.h2d_bytes = 0;  // the requests are kernel arguments
-    s->stats.d2h_bytes = size_t(N) * sizeof(yd_grant) + 8;  // written by the kernel into pinned host memory
-    s->have_stats = true;
-    if (s->debug_env) {
-      fprintf(stderr, "ydsched: solve n %u tiny 1 solver 3 spec 0 ring_cap %llu ring_lo %llu solve_ms %.3f\n", N,
-              (unsigned long long)s->ring_cap, (unsigned long long)s->lo, ms);
-    }
-    return;
-  }
+  if (TinySolve(s, now_ns, reqs, reqs16, N, out, out8, ids)) return;
 
   // Size classes: grids, scratch arrays and memsets are dimensioned for the next power of
   // two; kernels read the exact n from DynParams.
   const uint32_t Nb = (uint32_t)NextPow2(N, 1024);
   // The slot table: kept across solves (all running_tasks values of every servant) while it is small enough,
   // else rebuilt per solve and clamped to the batch size.
-  const size_t static_bound = S ? s->static_bound_cache : 0;  // (= StaticSlotBound(s), kept by SyncFacts)
+  const size_t static_bound = S ? s->static_bound_cache : 0;  // (kept by SyncFacts)
   const bool want_static = s->solver_pref != 1 && static_bound <= kStaticSlotLimit;
   size_t slot_bound = static_bound;
   if (!want_static) {
@@ -1527,7 +1754,6 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
   if (slot_bound > 0x7ffffff0ull) { fprintf(stderr, "ydsched: slot table too large\n"); abort(); }
   const size_t slot_b = (size_t)NextPow2(std::max<size_t>(slot_bound, 1), 4096);
   if (!want_static) s->order_static = false;
-  const uint32_t nb = (Nb + 1023) / 1024;
   EnsureSolveBuffers(s, Nb, slot_b);
   if (reqs16) s->d_reqs16.ensure(size_t(Nb) * sizeof(yd_task_req16));
   if (out8) s->d_out8.ensure(size_t(Nb) * sizeof(yd_grant8));
@@ -1542,68 +1768,38 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
   s->fsc.dyn = SetDynParams(s, N, N, now_ns);
 
   uint32_t launches = 0;
-  hp[1] = hp_now();
+  hp.Stamp(1);
   YD_CUDA_CHECK(cudaEventRecord(s->ev[0], st));
   // The request upload runs on its own stream so that the slot table and its sort (which
   // do not read the requests) overlap it; consumers wait on ev_h2d, recorded after the copy.
   // (Page-locked caller arrays -- yd_alloc_host -- are not copied at all when the fused kernel runs: its first phase
   // reads the requests over PCIe itself and, solo, its last phase writes the grants straight into the caller's array.
   // Staged requests are in HBM already.  Neither waits for the copy stream.)
-  bool uploaded = false, copied = false;
-  auto upload = [&]() {
-    if (uploaded) return;
-    if (reqs) {
-      YD_CUDA_CHECK(cudaMemcpyAsync(s->d_reqs.p, reqs, size_t(N) * sizeof(yd_task_req), cudaMemcpyHostToDevice, s->st_copy));
-      copied = true;
-    } else if (reqs16) {
-      YD_CUDA_CHECK(cudaMemcpyAsync(s->d_reqs16.p, reqs16, size_t(N) * sizeof(yd_task_req16), cudaMemcpyHostToDevice, s->st_copy));
-      copied = true;
-    }
-    if (copied) YD_CUDA_CHECK(cudaEventRecord(s->ev_h2d, s->st_copy));
-    uploaded = true;
-  };
-  auto mapped_address = [&](const void* p) -> void* {
-    if (!p || (reinterpret_cast<uintptr_t>(p) & 15u)) return nullptr;  // (16-byte vector accesses)
-    cudaPointerAttributes at{};
-    if (cudaPointerGetAttributes(&at, p) != cudaSuccess) { cudaGetLastError(); return nullptr; }
-    return at.type == cudaMemoryTypeHost ? at.devicePointer : nullptr;
-  };
+  bool copied = false;
   const void* in_host = reqs ? static_cast<const void*>(reqs) : static_cast<const void*>(reqs16);
-  void* const in_dev = mapped_address(in_host);
-  void* const out_dev = mapped_address(out ? static_cast<void*>(out) : static_cast<void*>(out8));
+  void* const in_dev = MappedAddress(in_host);
+  void* const out_dev = MappedAddress(out ? static_cast<void*>(out) : static_cast<void*>(out8));
   if (in_host) s->staged_n = 0;  // the staging area now holds this batch
-  bool graphed = false;
-  int merge_retry = 0, grow_attempts = 0;
-  uint32_t spec = 0;  // the speculative variant: 0 not tried, 1 decided the batch, 2 missed (the batch was replayed)
+  StandDowns downs;
   for (;;) {
     memset(s->h_meta.p, 0, 32);
-    graphed = false;
     // every buffer the sequence touches exists BEFORE a capture (no allocation inside one), and the scratch layout the
     // kept signature below describes is fixed
     if (plan.solver == 2) PrepareStreamBuffers(s, Nb, slot_b);
     const SolveGeometry geo = MakeGeometry(s, Nb, slot_b);
-    // The fused front kernel takes batches in the latency-bound regime whose (class, tile) count matrices one block
-    // scans in a few rounds; it needs the kept slot order.  Solo = it also writes the grants (no coupled component
-    // had requests last time; if one has now, the kernel raises flag 4 and the batch is replayed with kFused).
-    const bool fused = s->fused_cfg && s->fused_grid && s->solver_pref == 0 && plan.solver == 2 && want_static && S &&
-                       s->n_comps && Nb <= s->fused_max_nb && size_t(s->cls_bound) * geo.n_rtiles <= 32768 &&
-                       size_t(s->cls_bound) * geo.n_ltiles <= 32768;
     KeptSig now;
-    if (fused && s->solo.hint) {
-      now = KeptSig{CleanSig{g_buf_generation, s->z_cls_off, s->z_bytes, s->res_words, s->d_zero.p, s->d_res.p},
-                    s->topo_gen, s->cls_bound};
-    }
-    // speculative (fused.cuh): every block holds at most two request tiles (their classes and ranks stay in
-    // registers), the lists' offsets fit in shared memory, and registry positions fit the member words below the slot's
-    // index in its tile (classes.cuh: kMemberSlotShift)
-    const bool spec_ok = FusedLoffWords(s, geo) != 0 && geo.n_rtiles <= 2 * s->fused_grid && S <= yd::kMemberPosMask;
-    plan.variant = s->solo.Choose(fused, now, spec_ok);
+    plan.variant = ChooseVariant(s, Nb, geo, plan.solver, want_static, now);
     // (a staged solve -- no request array in this call -- leaves its grants in HBM and copies them afterwards, so that
     // the device-side events around it time the solve alone)
     const bool solo = IsSolo(plan.variant);
     const bool zc_in = plan.variant != kPipeline && in_dev, zc_out = solo && out_dev && in_host;
-    hp[2] = hp_now();
-    if (!zc_in) upload();
+    hp.Stamp(2);
+    if (!zc_in && in_host && !copied) {
+      YD_CUDA_CHECK(cudaMemcpyAsync(reqs ? s->d_reqs.p : s->d_reqs16.p, in_host,
+                                    size_t(N) * (reqs ? sizeof(yd_task_req) : sizeof(yd_task_req16)), cudaMemcpyHostToDevice, s->st_copy));
+      YD_CUDA_CHECK(cudaEventRecord(s->ev_h2d, s->st_copy));
+      copied = true;
+    }
     s->fsc.zc_in = zc_in ? in_dev : nullptr;
     s->fsc.zc_out = zc_out ? out_dev : nullptr;
     s->fsc.seq += 1;
@@ -1613,175 +1809,32 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
     if (plan.solver == 2 && want_static && S && s->n_comps && (s->order_dirty || !s->order_static || s->order_slot_b != slot_b)) {
       launches += RebuildSlotOrder(s, slot_b);
     }
-    if (solo) {
-      // ONE kernel whose per-call scalars are kernel parameters: launched directly, as a graph would add a parameter
-      // patch and a graph launch to the call.  Its arguments are built before the events, which bracket what the solve
-      // enqueues on `st`; the kernel leaves grant count and flags in the mapped host record.
-      const yd::FusedArgs a = MakeFusedArgs(s, Nb, geo, plan, false, packed & 1u, packed & 2u);
-      hp[3] = hp_now();
-      YD_CUDA_CHECK(cudaEventRecord(s->ev[1], st));
-      if (plan.variant == kSolo) {
-        // the solo kernel keeps the verdicts in registers: only the class-table keys behind res[] are initialised --
-        // and not even those when the previous solo solve left the scratch clean (kSoloClean, kSoloSpec)
-        YD_CUDA_CHECK(cudaMemsetAsync(s->d_res.as<uint32_t>() + s->res_words, 0xFF, yd::kClsTableSize * 8, st));
-        YD_CUDA_CHECK(cudaMemsetAsync(static_cast<char*>(s->d_zero.p) + s->z_cls_off, 0, s->z_bytes - s->z_cls_off, st));
-      }
-      WaitUpload(s, st, copied, false);
-      LaunchFusedKernel(s, a);
-      YD_CUDA_CHECK(cudaEventRecord(s->ev[4], st));
-      hp[4] = hp_now();
-      YD_CUDA_CHECK(cudaGetLastError());
-      launches += 1;
-    } else if (s->use_graphs) {
-      yd_sched::GraphKey key;
-      key.Nb = Nb; key.S = S; key.n_comps = s->n_comps; key.max_comp = s->max_comp_servants;
-      key.cls_bound = s->cls_bound; key.solver = plan.solver; key.wide = s->wide; key.slot_b = slot_b;
-      key.gen = g_buf_generation; key.topo_gen = s->topo_gen; key.ring_cap = s->ring_cap;
-      key.merge_rounds = plan.merge_rounds; key.force_stream = plan.force_stream;
-      key.order_static = (plan.solver == 2 && s->order_static) ? 1u : 0u;
-      key.variant = plan.variant; key.packed = packed;
-      yd_sched::GraphEntry* hit = nullptr;
-      for (auto& g : s->graphs) if (g.key == key) { hit = &g; break; }
-      if (!hit) {
-        cudaGraph_t graph = nullptr;
-        YD_CUDA_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-        uint32_t l = EnqueueSolve(s, Nb, geo, plan, false, copied, true, packed);
-        YD_CUDA_CHECK(cudaStreamEndCapture(st, &graph));
-        cudaGraphExec_t exec = nullptr;
-        YD_CUDA_CHECK(cudaGraphInstantiate(&exec, graph, 0));
-        YD_CUDA_CHECK(cudaGraphDestroy(graph));
-        if (s->graphs.size() >= 16) {  // drop the oldest size class
-          cudaGraphExecDestroy(s->graphs.front().exec);
-          s->graphs.erase(s->graphs.begin());
-        }
-        s->graphs.push_back(yd_sched::GraphEntry{key, exec, l});
-        hit = &s->graphs.back();
-      }
-      hp[3] = hp_now();
-      YD_CUDA_CHECK(cudaEventRecord(s->ev[1], st));
-      YD_CUDA_CHECK(cudaGraphLaunch(hit->exec, st));
-      YD_CUDA_CHECK(cudaEventRecord(s->ev[4], st));
-      hp[4] = hp_now();
-      launches += hit->launches;
-      graphed = true;
-    } else {
-      launches += EnqueueSolve(s, Nb, geo, plan, true, copied, false, packed);
-    }
+    if (solo) launches += LaunchSolo(s, Nb, geo, plan, copied, packed, hp);
+    else if (s->use_graphs) launches += LaunchGraphed(s, Nb, slot_b, geo, plan, copied, packed, hp);
+    else launches += EnqueueSolve(s, Nb, geo, plan, true, copied, false, packed);
     if (plan.solver == 1) { s->order_dirty = true; s->order_static = false; }  // the row-scan solver's table overwrote the kept one
     if (zc_out) {}  // the kernel wrote the grants into the caller's page-locked array
     else if (out8) YD_CUDA_CHECK(cudaMemcpyAsync(out8, s->d_out8.p, size_t(N) * sizeof(yd_grant8), cudaMemcpyDeviceToHost, st));
     else YD_CUDA_CHECK(cudaMemcpyAsync(out, s->d_out.p, size_t(N) * sizeof(yd_grant), cudaMemcpyDeviceToHost, st));
     YD_CUDA_CHECK(cudaEventRecord(s->ev[5], st));
-    hp[5] = hp_now();
+    hp.Stamp(5);
     YD_CUDA_CHECK(cudaStreamSynchronize(st));
-    hp[6] = hp_now();
+    hp.Stamp(6);
     if (solo) {  // the solo kernel's report: flags and grant count (no copy follows its launch)
       if (s->h_fio->done_seq != s->fsc.seq) { fprintf(stderr, "ydsched: the fused kernel left no report\n"); abort(); }
       memcpy(s->h_meta.p, const_cast<const uint32_t*>(s->h_fio->meta), 32);
       s->h_counters.as<Counters>()->granted = s->h_fio->granted;
     }
-    if (s->fused_prof && plan.variant == kSoloSpec) {
-      unsigned long long t[9];
-      YD_CUDA_CHECK(cudaMemcpy(t, s->d_fused_prof.p, sizeof t, cudaMemcpyDeviceToHost));
-      if (s->h_meta.as<uint32_t>()[1] == yd::kFlagSpecMiss) {  // (no phase B)
-        fprintf(stderr, "ydsched: fused variant 4 (speculative) n %u ns: A %llu barrier %llu missed\n", N, t[1] - t[0], t[2] - t[1]);
-      } else {
-        fprintf(stderr, "ydsched: fused variant 4 (speculative) n %u ns: A %llu barrier %llu B %llu total %llu (+tail %lld)\n", N,
-                t[1] - t[0], t[2] - t[1], t[7] - t[2], t[7] - t[0], (long long)(t[8] - t[7]));
-      }
-      // every block's stamps (fused.cuh: kProfBlockWords), for tools/dev/phase_prof.py
-      const uint32_t G = s->fused_grid;
-      std::vector<unsigned long long> b(size_t(G) * yd::kProfBlockWords);
-      YD_CUDA_CHECK(cudaMemcpy(b.data(), s->d_fused_prof.as<unsigned long long>() + yd::kProfHead, b.size() * 8,
-                               cudaMemcpyDeviceToHost));
-      std::string line = "ydsched: fused blocks " + std::to_string(G) + " last_end " + std::to_string(t[8]) + " stamps";
-      for (unsigned long long v : b) line += " " + std::to_string(v);
-      fprintf(stderr, "%s\n", line.c_str());
-    } else if (s->fused_prof && plan.variant != kPipeline) {
-      unsigned long long t[9];
-      YD_CUDA_CHECK(cudaMemcpy(t, s->d_fused_prof.p, sizeof t, cudaMemcpyDeviceToHost));
-      fprintf(stderr, "ydsched: fused variant %u n %u ns: P1 %llu E1 %llu P3 %llu E2 %llu P5 %llu B3 %llu P6 %llu total %llu (+report/clean %lld)\n",
-              (unsigned)plan.variant, N, t[1] - t[0], t[2] - t[1], t[3] - t[2], t[4] - t[3], t[5] - t[4], t[6] - t[5], t[7] - t[6],
-              t[7] - t[0], (long long)(t[8] - t[7]));
-    }
-    const uint32_t* meta = s->h_meta.as<uint32_t>();
-    s->solo.Take(plan.variant, meta, now, s->h_fio->classes_fp);
-    if (plan.solver == 2 && S && s->n_comps && meta[1] != 0) {
-      // Nothing was decided (the stream solver and the final kernels all stood down).
-      const uint32_t flag = meta[1];
-      if (flag == yd::kFlagSpecMiss) {
-        // the kept class table could not decide the batch: replay without speculation (which builds the table again)
-        spec = 2;
-      } else if (flag == 4) {
-        // the solo kernel met a component it cannot decide: the general sequence, now and next time (SoloTables::Take)
-      } else if (flag == 2 && grow_attempts++ < 3 && GrowClassBound(s, meta)) {
-        // more lists than provisioned: go again with the grown class bound
-      } else if (flag == 3 && merge_retry < 2) {
-        // the merge solver's boundary states had not settled after the rounds in the graph: more
-        // rounds first, then the sequential solver for everything it would have decided
-        if (merge_retry == 0) plan.MoreMergeRounds(s->merge_max_chunks);
-        else plan.force_stream = 2;
-        ++merge_retry;
-      } else {
-        if (s->max_comp_servants > kRowscanMaxComponent) {
-          // More classes than the class table holds AND a component beyond the row-scan solver's reach.  n sequential
-          // decisions are the first half's followed by the second half's: decide the batch as two consecutive halves
-          // (each with half the requests, hence -- eventually -- few enough classes).
-          if (N < 2) { fprintf(stderr, "ydsched: class table overflow on a single request\n"); abort(); }
-          std::vector<yd_task_req> r(N);
-          if (reqs) memcpy(r.data(), reqs, size_t(N) * sizeof(yd_task_req));
-          else if (reqs16) for (uint32_t i = 0; i != N; ++i) r[i] = yd_unpack_req(reqs16[i]);
-          else YD_CUDA_CHECK(cudaMemcpy(r.data(), s->d_reqs.p, size_t(N) * sizeof(yd_task_req), cudaMemcpyDeviceToHost));
-          std::vector<yd_grant> g(N);
-          const uint32_t h = N / 2;
-          WaitImpl(s, now_ns, r.data(), nullptr, h, g.data(), nullptr, nullptr);
-          WaitImpl(s, now_ns, r.data() + h, nullptr, N - h, g.data() + h, nullptr, nullptr);
-          if (out) memcpy(out, g.data(), size_t(N) * sizeof(yd_grant));
-          else for (uint32_t i = 0; i != N; ++i) out8[i] = yd_pack_grant(g[i], *ids_out);
-          s->stats.decisions = N;
-          return;
-        }
-        plan.solver = 1;
-      }
-      continue;
-    }
-    if (plan.variant == kSoloSpec) spec = 1;
-    break;
+    if (s->fused_prof) PrintFusedProfile(s, plan.variant, N);
+    s->solo.Take(plan.variant, s->h_meta.as<uint32_t>(), now, s->h_fio->classes_fp);
+    const AttemptEnd end = StandDown(s, plan, downs);
+    if (end == kHalves) return SolveInHalves(s, now_ns, reqs, reqs16, N, out, out8, ids);
+    if (end == kDecided) break;
   }
-  const Counters* c = s->h_counters.as<Counters>();
-  s->next_id += c->granted;
-
-  yd_solve_stats& stt = s->stats;
-  stt = yd_solve_stats{};
-  // (the event arithmetic costs a driver call apiece: done when yd_last_solve_stats asks, the events stay valid until the next solve)
-  s->stats_times_pending = (graphed || IsSolo(plan.variant)) ? 2 : 1;
-  stt.decisions = N;
-  stt.granted = c->granted;
-  stt.kernel_launches = launches;
-  stt.solver = plan.solver;
-  stt.h2d_bytes = (reqs ? size_t(N) * sizeof(yd_task_req) : reqs16 ? size_t(N) * sizeof(yd_task_req16) : 0) + sizeof(yd::DynParams);
-  stt.d2h_bytes = size_t(N) * (out8 ? sizeof(yd_grant8) : sizeof(yd_grant)) + sizeof(Counters) + 32;
-  s->have_stats = true;
-  if (s->host_prof) {
-    hp[7] = hp_now();
-    fprintf(stderr, "ydsched: host us: prep %.1f (attrs+variant %.1f) upload+prep %.1f launch %.1f d2h-enqueue %.1f sync-wait %.1f stats %.1f total %.1f\n",
-            hp[1] - hp[0], hp[2] - hp[1], hp[3] - hp[2], hp[4] - hp[3], hp[5] - hp[4], hp[6] - hp[5], hp[7] - hp[6], hp[7] - hp[0]);
-  }
-  if (s->debug_env) {
-    // which path the solve took (the last attempt, after any stand-down): `final` 0 = the solo kernel wrote the grants,
-    // 1 = k_final_fused, 3 = k_final_count / k_final_scan / k_final_write; `spec` over all attempts; the lease ring
-    // (`ring_lo` = the first live id) as the solve found it
-    const bool have_work = S && s->n_comps;
-    const uint32_t solver = plan.solver;
-    const uint32_t final_path = (IsSolo(plan.variant) && have_work && solver == 2) ? 0u : (solver == 2 && have_work && nb <= 2048) ? 1u : 3u;
-    const auto back = solver == 2 && have_work && !IsSolo(plan.variant) ? MergeBack(s) : std::pair<uint32_t, uint32_t>{0, 0};
-    fprintf(stderr, "ydsched: solve n %u tiny 0 variant %u order_static %d wide %d Nb %u slot_b %zu cls_bound %u final %u "
-            "emask %d max_comp %zu solver %u graph %d merge_rounds %llu merge_chunks %llu walks %llu windows %llu "
-            "merge_back %u merge_back_n %u spec %u ring_cap %llu ring_lo %llu solve_ms %.3f\n",
-            N, (unsigned)plan.variant, (int)(solver == 2 && s->order_static), (int)s->wide, Nb, slot_b, s->cls_bound, final_path,
-            (int)s->emask_ok, (size_t)s->max_comp_servants, solver, (int)graphed, c->pad[0], c->pad[1], c->pad[2],
-            c->pad[3], back.first, back.second, spec, (unsigned long long)s->ring_cap, (unsigned long long)s->lo, stt.solve_ms);
-  }
+  s->next_id += s->h_counters.as<Counters>()->granted;
+  RecordSolveStats(s, N, launches, plan, reqs, reqs16, out8);
+  hp.Print();
+  if (s->debug_env) PrintSolveLine(s, N, Nb, slot_b, plan, downs.spec);
 }
 }  // namespace
 }  // extern "C++"
@@ -1795,8 +1848,7 @@ void yd_wait_for_starting_new_tasks(yd_sched* s, int64_t now_ns, const yd_task_r
 // The same decisions with 16-byte requests up and 8-byte grants down (ydsched.h: yd_task_req16, yd_grant8).
 void yd_wait_for_starting_new_tasks_packed(yd_sched* s, int64_t now_ns, const yd_task_req16* reqs, size_t n,
                                            yd_grant8* out, yd_packed_ids* ids) {
-  yd_packed_ids local;
-  WaitImpl(s, now_ns, nullptr, reqs, n, nullptr, out, ids ? ids : &local);
+  WaitImpl(s, now_ns, nullptr, reqs, n, nullptr, out, ids);
 }
 
 extern "C++" {
@@ -2152,7 +2204,7 @@ int yd_get_servant_personality(yd_sched* s, uint32_t idx, yd_servant* out) {
   return 1;
 }
 
-uint64_t yd_next_task_id(yd_sched* s) { return s->next_id * s->id_stride + s->id_offset; }
+uint64_t yd_next_task_id(yd_sched* s) { return BatchIds(s).first_task_id; }
 
 uint64_t yd_num_tasks(yd_sched* s) {
   YD_CUDA_CHECK(cudaSetDevice(s->device));
@@ -2389,9 +2441,6 @@ static void FilterPrepare(yd_sched* s, uint32_t N, bool bloom, size_t key_span, 
   }
 }
 
-// What turns the packed grants of the next batch into task ids (yd_packed_ids).
-static yd_packed_ids BatchIds(const yd_sched* s) { return yd_packed_ids{s->next_id * s->id_stride + s->id_offset, s->id_stride}; }
-
 // The pre-filters' keys on the device (d_bloom_keys, d_rt_keys): fixed-length records of len bytes at a stride
 // (yd_prefilter), or with `binary` contiguous 32-byte digests (yd_prefilter_packed).
 struct FilterKeys {
@@ -2471,9 +2520,7 @@ static size_t FilterStages(yd_sched* s, int64_t now_ns, uint32_t N, const Filter
     yd_last_solve_stats(s, &st2);  // (turns the solve's events into milliseconds before they are reused)
   } else {
     if (ids) *ids = BatchIds(s);
-    s->stats = yd_solve_stats{};
-    s->stats_times_pending = 0;
-    s->have_stats = true;
+    ResetStats(s);
   }
   // stats of the whole call: prep = the filter stages + compaction (device), solve / final = the solve's, decisions = n
   s->stats.prep_ms += filter_ms;
@@ -2497,7 +2544,7 @@ static size_t FilterCall(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, c
     if (ids) *ids = BatchIds(s);
     return 0;
   }
-  if (n > 0x40000000ull) { fprintf(stderr, "ydsched: batch too large\n"); abort(); }
+  CheckBatchSize(n);
   YD_CUDA_CHECK(cudaSetDevice(s->device));
   cudaStream_t st = s->st;
   const uint32_t N = (uint32_t)n;
@@ -2542,9 +2589,7 @@ size_t yd_filter_and_wait_for_starting_new_tasks_packed(yd_sched* s, int64_t now
                                                         const yd_prefilter_packed* filter, uint8_t* verdict_out,
                                                         yd_running_hit* hits_out, yd_grant8* grants_out,
                                                         yd_packed_ids* ids) {
-  yd_packed_ids local;
-  return FilterCall(s, now_ns, nullptr, reqs, n, nullptr, filter, verdict_out, hits_out, nullptr, grants_out,
-                    ids ? ids : &local, false);
+  return FilterCall(s, now_ns, nullptr, reqs, n, nullptr, filter, verdict_out, hits_out, nullptr, grants_out, ids, false);
 }
 
 // ---- cache keys and task digests from task descriptors (blake3.cuh) ------------------------------------------------
@@ -2640,7 +2685,7 @@ int yd_derive_task_keys(yd_sched* s, const yd_task_req* reqs, size_t n, const yd
                         char* task_digests_out) {
   if (int rc = yd_keys_check(s->envs, reqs, n, src)) return rc;
   if (n == 0 || (!cache_keys_out && !task_digests_out)) return YD_KEYS_OK;
-  if (n > 0x40000000ull) { fprintf(stderr, "ydsched: batch too large\n"); abort(); }
+  CheckBatchSize(n);
   YD_CUDA_CHECK(cudaSetDevice(s->device));
   cudaStream_t st = s->st;
   const size_t kb = cache_keys_out ? n * YD_KEYS_CACHE_KEY_LEN : 0, db = task_digests_out ? n * YD_KEYS_TASK_DIGEST_LEN : 0;
@@ -2663,7 +2708,7 @@ static size_t DeriveFilterCall(yd_sched* s, int64_t now_ns, const yd_task_req* r
                                uint32_t stages, uint8_t* verdict_out, yd_running_hit* hits_out, yd_grant* grants_out,
                                bool group) {
   if (n == 0) return group ? ShardSolveKept(s, now_ns, 0, 0, false, grants_out, nullptr, nullptr) : 0;
-  if (n > 0x40000000ull) { fprintf(stderr, "ydsched: batch too large\n"); abort(); }
+  CheckBatchSize(n);
   const bool bloom = stages & YD_STAGE_CACHE, dedupe = stages & YD_STAGE_DEDUPE;
   if (bloom && !s->bloom_bits) { fprintf(stderr, "ydsched: bloom filter used before yd_bloom_reset / yd_bloom_load\n"); abort(); }
   YD_CUDA_CHECK(cudaSetDevice(s->device));

@@ -18,17 +18,17 @@ all: cuda oracle fake_nccl primitives
 
 cuda: $(LIB)
 
-$(LIB): include/ydstate.h include/ydkeys.h include/ydstate_codec.inc include/yddump_impl.inc include/ydsched_keys_impl.inc $(CSRC)/ydsched.cu $(wildcard $(CSRC)/*.cuh) $(wildcard $(CSRC)/*.inc) include/ydshard.h include/ydfilter_packed.h include/ydruns.h include/ydsched.h include/ydsched_rpc_impl.inc include/ydservice.h include/ydservice_impl.inc include/ydwire.h include/ydwire_impl.inc
+$(LIB): include/ydstate.h include/ydkeys.h include/ydstate_codec.inc include/yddump_impl.inc include/ydsched_keys_impl.inc $(CSRC)/ydsched.cu $(wildcard $(CSRC)/*.cuh) $(wildcard $(CSRC)/*.inc) include/ydshard.h include/ydfilter_packed.h include/ydrpcs_packed.h include/ydruns.h include/ydsched.h include/ydsched_rpc_impl.inc include/ydservice.h include/ydservice_impl.inc include/ydwire.h include/ydwire_impl.inc
 	$(NVCC) $(NVCCFLAGS) $(PTXAS_V) -shared -o $@ $(CSRC)/ydsched.cu -ldl
 
 oracle: checkers/libydport_state.so checkers/libydport_keys.so
 	$(MAKE) -C oracle all
 	$(MAKE) -C oracle -f keys.mk all
 
-checkers/libydport_state.so: checkers/port_state.cc oracle/port.cc include/ydstate.h include/ydstate_codec.inc include/ydsched.h include/ydfilter_packed.h include/ydruns.h $(wildcard include/*.inc)
+checkers/libydport_state.so: checkers/port_state.cc oracle/port.cc include/ydstate.h include/ydstate_codec.inc include/ydsched.h include/ydfilter_packed.h include/ydrpcs_packed.h include/ydruns.h $(wildcard include/*.inc)
 	$(CXX) -std=gnu++2a -O2 -fPIC -Wall -Wno-sign-compare -Wno-unused-variable -Wno-subobject-linkage -Iinclude -shared -o $@ checkers/port_state.cc
 
-checkers/libydport_keys.so: checkers/port_keys.cc oracle/port.cc include/ydsched.h include/ydkeys.h include/ydfilter_packed.h include/ydruns.h $(wildcard include/*.inc)
+checkers/libydport_keys.so: checkers/port_keys.cc oracle/port.cc include/ydsched.h include/ydkeys.h include/ydfilter_packed.h include/ydrpcs_packed.h include/ydruns.h $(wildcard include/*.inc)
 	$(CXX) -std=gnu++2a -O2 -fPIC -Wall -Wno-sign-compare -Wno-unused-variable -Wno-subobject-linkage -Iinclude -shared -o $@ checkers/port_keys.cc
 
 FAKE_NCCL = tests/fake_nccl/libnccl.so.2

@@ -29,6 +29,7 @@
 
 #include "ydfilter_packed.h"
 #include "ydkeys.h"
+#include "ydrpcs_packed.h"
 #include "ydsched.h"
 #include "ydservice.h"
 
@@ -135,6 +136,15 @@ size_t yd_shard_running_index_refresh(yd_sched* s);
  * batch above 2^30 decisions, or capacities above 8192 per servant) happens on every rank and decides nothing. */
 size_t yd_shard_wait_for_starting_task_rpcs(yd_sched* s, int64_t now_ns, const yd_rpc_wait* rpcs, size_t n_rpcs,
                                             yd_rpc_wait_result* results, yd_grant* grants_out, size_t cap);
+/* yd_shard_wait_for_starting_task_rpcs with 8-byte grants (ydrpcs_packed.h): defined as that call, then yd_pack_grant of
+ * every grant with the group batch's *ids (the same on every rank).  Every rank returns the same results, grants and
+ * *ids, and its refusals (those of the unpacked group call, and of yd_wait_for_starting_task_rpcs_packed) happen on every
+ * rank.  Every rank expands its own even range of the window on the device, decides it with the packed sharded solve,
+ * and one all-gather of the 8-byte grants (device to device) gives every rank the whole window to report.  On a handle
+ * that has not joined a group, this is the single-handle call. */
+size_t yd_shard_wait_for_starting_task_rpcs_packed(yd_sched* s, int64_t now_ns, const yd_rpc_wait* rpcs, size_t n_rpcs,
+                                                   yd_rpc_wait_result* results, yd_grant8* grants_out, size_t cap,
+                                                   yd_packed_ids* ids);
 /* A SchedulerServiceImpl over the group (ydservice.h; ydwire.h works on it unchanged).  Collective; every rank passes the
  * same config.  Its handlers make the replicated calls above: Heartbeat's notification, WaitForStartingTask,
  * KeepTaskAlive, GetRunningTasks, and FreeTask through yd_shard_free_tasks (rank 0 passes the ids).  KeepServantAlive is

@@ -296,9 +296,10 @@ def load_library(path: os.PathLike | str | None = None) -> C.CDLL:
         if fn is not None:
             fn.restype = restype
             fn.argtypes = argtypes
-    # include/ydshard.h: only the CUDA library has the range-sharded multi-GPU path; include/ydfilter_packed.h and
-    # include/ydruns.h: the CPU checkers export them from builds of their own (the product library must export all)
-    for name, restype, argtypes in SHARD_PROTOTYPES + FILTER_PACKED_PROTOTYPES + RUNS_PROTOTYPES:
+    # include/ydshard.h: only the CUDA library has the range-sharded multi-GPU path; include/ydfilter_packed.h,
+    # include/ydrpcs_packed.h and include/ydruns.h: the CPU checkers export them from builds of their own (the product
+    # library must export all)
+    for name, restype, argtypes in SHARD_PROTOTYPES + FILTER_PACKED_PROTOTYPES + RPCS_PACKED_PROTOTYPES + RUNS_PROTOTYPES:
         fn = getattr(lib, name) if path is None else getattr(lib, name, None)
         if fn is not None:
             fn.restype = restype
@@ -345,6 +346,7 @@ SHARD_PROTOTYPES = [
      [_P, C.c_int64, _P, C.c_size_t, _P, C.c_uint32, _P, _P, _P]),
     ("yd_shard_filter_and_wait_for_starting_new_tasks_packed", C.c_size_t,
      [_P, C.c_int64, _P, C.c_size_t, _P, _P, _P, _P, _P]),
+    ("yd_shard_wait_for_starting_task_rpcs_packed", C.c_size_t, [_P, C.c_int64, _P, C.c_size_t, _P, _P, C.c_size_t, _P]),
 ]
 
 # Every symbol include/ydstate.h declares, and its status codes.
@@ -352,6 +354,11 @@ SHARD_PROTOTYPES = [
 FILTER_PACKED_PROTOTYPES = [
     ("yd_filter_and_wait_for_starting_new_tasks_packed", C.c_size_t,
      [_P, C.c_int64, _P, C.c_size_t, _P, _P, _P, _P, _P]),
+]
+
+# include/ydrpcs_packed.h: a window of WaitForStartingTask RPCs with 8-byte grants.
+RPCS_PACKED_PROTOTYPES = [
+    ("yd_wait_for_starting_task_rpcs_packed", C.c_size_t, [_P, C.c_int64, _P, C.c_size_t, _P, _P, C.c_size_t, _P]),
 ]
 
 # include/ydkeys.h: the task keys, exported by the CUDA library and by the checkers' builds that have them

@@ -38,12 +38,14 @@
 #include "tiny.cuh"
 #include "fused.cuh"
 #include "filter.cuh"
+#include "rpcs.cuh"
 #include "blake3.cuh"
 #include "state.cuh"
 #include "ydstate_codec.inc"
 #include "ydkeys.h"
 #include "ydshard.h"
 #include "ydruns.h"
+#include "ydrpcs_packed.h"
 #include "ydsched_keys_impl.inc"
 
 namespace {
@@ -363,6 +365,9 @@ struct yd_sched {
   std::vector<RunningRec> rt_snapshot;
   DevBuf d_rt_bytes, d_rt_off, d_rt_len, d_rt_ids, d_rt_slots, d_rt_keys, d_rt_out;
   DevBuf d_freqs, d_fverdict, d_ftile;  // pre-filtered solve (filter.cuh): the unfiltered queue, verdicts, tile counts
+  // a window of RPCs decided on the device (rpcs.cuh): the records, where each RPC's decisions start, its grant counts
+  // (scanned: first_grant), the results, the reported grants
+  DevBuf d_rpcs, d_rpc_off, d_rpc_ng, d_rpc_res, d_rpc_out;
   PinBuf h_fcount;
   cudaEvent_t ev_f[2] = {};
   // the env table on the device (blake3.cuh): digest e = env_bytes[env_off[e] .. env_off[e + 1]) for e < env_dev_n,
@@ -748,7 +753,10 @@ void yd_destroy(yd_sched* s) {
   for (PinBuf* b : {&s->h_facts, &s->h_topo, &s->h_counters, &s->h_small, &s->h_dyn, &s->h_meta, &s->h_fsc}) b->release();
   for (auto& e : s->ev) cudaEventDestroy(e);
   for (auto& e : s->ev_f) cudaEventDestroy(e);
-  for (DevBuf* b : {&s->d_freqs, &s->d_fverdict, &s->d_ftile}) b->release();
+  for (DevBuf* b : {&s->d_freqs, &s->d_fverdict, &s->d_ftile, &s->d_rpcs, &s->d_rpc_off, &s->d_rpc_ng, &s->d_rpc_res,
+                    &s->d_rpc_out}) {
+    b->release();
+  }
   if (s->d_env_bytes) cudaFree(s->d_env_bytes);
   if (s->d_env_off) cudaFree(s->d_env_off);
   s->h_fcount.release();
@@ -1371,6 +1379,17 @@ void WriteGrants(yd_grant* out, yd_grant8* out8, const yd_packed_ids& ids, const
   else if (n) memcpy(out, g, n * sizeof(yd_grant));
 }
 
+// n grants packed with `ids` into d_out8, for a device-side consumer (`keep8` of WaitImpl and ShardSolve): the grants
+// of the paths that decide on the host side of the device (halves, the group's whole-queue fallback, no servants).
+void UploadGrants8(yd_sched* s, const yd_packed_ids& ids, const yd_grant* g, size_t n) {
+  if (!n) return;
+  std::vector<yd_grant8> g8(n);
+  for (size_t i = 0; i != n; ++i) g8[i] = yd_pack_grant(g[i], ids);
+  s->d_out8.ensure(n * sizeof(yd_grant8));
+  YD_CUDA_CHECK(cudaMemcpyAsync(s->d_out8.p, g8.data(), n * sizeof(yd_grant8), cudaMemcpyHostToDevice, s->st));
+  YD_CUDA_CHECK(cudaStreamSynchronize(s->st));
+}
+
 // Everything between the request upload and the grant download, for size class (Nb, slot_b), of a general (not solo)
 // solve: the sequence that is captured into a CUDA graph.  (A solo solve is one kernel: LaunchSolo launches it.)
 // packed bit 0: the upload is 16-byte records in d_reqs16; bit 1: the download is 8-byte grants from d_out8.
@@ -1672,7 +1691,7 @@ AttemptEnd StandDown(yd_sched* s, SolvePlan& plan, StandDowns& d) {
 // are the first half's followed by the second half's: decide the batch as two consecutive halves (each with half the
 // requests, hence -- eventually -- few enough classes).  The stats are the second half's, with decisions = N.
 void SolveInHalves(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_task_req16* reqs16, uint32_t N,
-                   yd_grant* out, yd_grant8* out8, const yd_packed_ids& ids) {
+                   yd_grant* out, yd_grant8* out8, const yd_packed_ids& ids, bool keep8) {
   if (N < 2) { fprintf(stderr, "ydsched: class table overflow on a single request\n"); abort(); }
   std::vector<yd_task_req> r(N);
   if (reqs || reqs16) CopyRequests(reqs, reqs16, N, r.data());
@@ -1681,7 +1700,8 @@ void SolveInHalves(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const y
   const uint32_t h = N / 2;
   yd_wait_for_starting_new_tasks(s, now_ns, r.data(), h, g.data());
   yd_wait_for_starting_new_tasks(s, now_ns, r.data() + h, N - h, g.data() + h);
-  WriteGrants(out, out8, ids, g.data(), N);
+  if (keep8) UploadGrants8(s, ids, g.data(), N);
+  else WriteGrants(out, out8, ids, g.data(), N);
   s->stats.decisions = N;
 }
 
@@ -1718,9 +1738,10 @@ void PrintSolveLine(yd_sched* s, uint32_t N, uint32_t Nb, size_t slot_b, const S
 
 // The solve behind yd_wait_for_starting_new_tasks and its packed twin.  Requests: `reqs` (24-byte records), or `reqs16`
 // (16-byte records), or neither = the first n staged requests (yd_stage_requests) are already in HBM.  Grants: `out`
-// (16-byte records) or `out8` (8-byte records, ids = first_task_id + ordinal * stride of BatchIds, also to ids_out).
+// (16-byte records) or `out8` (8-byte records, ids = first_task_id + ordinal * stride of BatchIds, also to ids_out), or
+// with `keep8` neither: the 8-byte records stay in d_out8 for a device-side consumer (the RPC window, rpcs.cuh).
 void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_task_req16* reqs16, size_t n, yd_grant* out,
-              yd_grant8* out8, yd_packed_ids* ids_out) {
+              yd_grant8* out8, yd_packed_ids* ids_out, bool keep8 = false) {
   const yd_packed_ids ids = BatchIds(s);
   if (ids_out) *ids_out = ids;
   if (n == 0) return;
@@ -1732,7 +1753,7 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
   cudaStream_t st = s->st;
   const uint32_t N = (uint32_t)n;
   const uint32_t S = (uint32_t)s->sv.size();
-  const uint32_t packed = (reqs16 ? 1u : 0u) | (out8 ? 2u : 0u);
+  const uint32_t packed = (reqs16 ? 1u : 0u) | (out8 || keep8 ? 2u : 0u);
   s->SyncServantState();
   s->SyncFacts();
   s->SyncTopology();
@@ -1756,7 +1777,7 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
   if (!want_static) s->order_static = false;
   EnsureSolveBuffers(s, Nb, slot_b);
   if (reqs16) s->d_reqs16.ensure(size_t(Nb) * sizeof(yd_task_req16));
-  if (out8) s->d_out8.ensure(size_t(Nb) * sizeof(yd_grant8));
+  if (out8 || keep8) s->d_out8.ensure(size_t(Nb) * sizeof(yd_grant8));
 
   // solver choice: 2 (slot streams) unless asked otherwise or a component is too big for it
   // (the slot-stream solver takes components of any size: its sequential fallback keeps running_tasks of a
@@ -1813,7 +1834,7 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
     else if (s->use_graphs) launches += LaunchGraphed(s, Nb, slot_b, geo, plan, copied, packed, hp);
     else launches += EnqueueSolve(s, Nb, geo, plan, true, copied, false, packed);
     if (plan.solver == 1) { s->order_dirty = true; s->order_static = false; }  // the row-scan solver's table overwrote the kept one
-    if (zc_out) {}  // the kernel wrote the grants into the caller's page-locked array
+    if (zc_out || keep8) {}  // the kernel wrote the grants into the caller's page-locked array, or they stay in HBM
     else if (out8) YD_CUDA_CHECK(cudaMemcpyAsync(out8, s->d_out8.p, size_t(N) * sizeof(yd_grant8), cudaMemcpyDeviceToHost, st));
     else YD_CUDA_CHECK(cudaMemcpyAsync(out, s->d_out.p, size_t(N) * sizeof(yd_grant), cudaMemcpyDeviceToHost, st));
     YD_CUDA_CHECK(cudaEventRecord(s->ev[5], st));
@@ -1828,7 +1849,7 @@ void WaitImpl(yd_sched* s, int64_t now_ns, const yd_task_req* reqs, const yd_tas
     if (s->fused_prof) PrintFusedProfile(s, plan.variant, N);
     s->solo.Take(plan.variant, s->h_meta.as<uint32_t>(), now, s->h_fio->classes_fp);
     const AttemptEnd end = StandDown(s, plan, downs);
-    if (end == kHalves) return SolveInHalves(s, now_ns, reqs, reqs16, N, out, out8, ids);
+    if (end == kHalves) return SolveInHalves(s, now_ns, reqs, reqs16, N, out, out8, ids, keep8);
     if (end == kDecided) break;
   }
   s->next_id += s->h_counters.as<Counters>()->granted;
@@ -2250,6 +2271,122 @@ void yd_free_host(void* p) {
 #include "yddump_impl.inc"
 #include "ydservice_impl.inc"
 #include "ydwire_impl.inc"
+
+// ---- a window of WaitForStartingTask RPCs decided on the device (include/ydrpcs_packed.h, rpcs.cuh) -----------------
+extern "C" {
+// The range-sharded group's part of a window (shard_host.inc).
+static std::vector<unsigned long long> ShardRanges(const yd_sched* s, size_t total, size_t* lo, size_t* hi);
+static int ShardDecideWindow(yd_sched* s, int64_t now_ns, const std::vector<unsigned long long>& counts);
+}  // extern "C"
+
+extern "C++" {
+namespace {
+bool ShardRefusesWide(yd_sched* s);  // (shard_host.inc)
+
+// Windows of at most this many decisions keep the host expansion: on the host their queue goes to the one-launch tiny
+// solve (k_solve_tiny, the requests as kernel arguments), which a staged queue cannot take, so expanding on the device
+// would trade that one launch for an upload, six launches and the general solve.
+constexpr size_t kHostWindowMax = yd::kTinyMax;
+
+// yd_wait_for_starting_task_rpcs_packed, and with `group` its range-sharded form.  The host computes the window's size
+// and its refusals (O(n_rpcs), nothing per decision) and uploads the RPC records; the device expands the window into the
+// staged queue (this handle's range of it), the staged solve decides it with its 8-byte grants left in HBM (on a group:
+// gathered from every rank, device to device), and the report writes the results and the grants in ordinal order.
+size_t RpcWindow(yd_sched* s, int64_t now_ns, const yd_rpc_wait* rpcs, size_t n_rpcs, yd_rpc_wait_result* results,
+                 yd_grant8* grants_out, size_t cap, yd_packed_ids* ids, bool group) {
+  const yd_packed_ids id0 = BatchIds(s);  // (a group's next_id is replicated)
+  if (ids) *ids = id0;
+  const size_t total = yd_rpc_expanded_requests(s, rpcs, n_rpcs);
+  if (!yd_rpc_detail::Fits(total, cap)) return (size_t)-1;
+  if (total == 0 || (!group && total <= kHostWindowMax) || n_rpcs >= 0x40000000ull) {
+    // the definition itself: the unpacked call, the grants packed
+    static thread_local yd_rpc_detail::HostStage stage;
+    yd_grant* g = static_cast<yd_grant*>(stage.ensure(std::max<size_t>(total, 1) * sizeof(yd_grant)));
+    if (!g) return (size_t)-1;
+    const size_t k = group ? yd_shard_wait_for_starting_task_rpcs(s, now_ns, rpcs, n_rpcs, results, g, cap)
+                           : yd_wait_for_starting_task_rpcs(s, now_ns, rpcs, n_rpcs, results, g, cap);
+    if (k != (size_t)-1) WriteGrants(nullptr, grants_out, id0, g, k);
+    return k;
+  }
+  if (group && ShardRefusesWide(s)) return (size_t)-1;  // (before anything changes, as the unpacked group call refuses)
+  YD_CUDA_CHECK(cudaSetDevice(s->device));
+  cudaStream_t st = s->st;
+  const uint64_t bound = yd_grant_capacity_bound(s);
+  const uint32_t n = (uint32_t)n_rpcs, T = (uint32_t)total;
+  // this handle's range [lo, hi) of the queue: all of it, or a group rank's (ShardRanges)
+  size_t lo = 0, hi = total;
+  std::vector<unsigned long long> counts;
+  if (group) counts = ShardRanges(s, total, &lo, &hi);
+  s->d_rpcs.ensure(n_rpcs * sizeof(yd_rpc_wait));
+  s->d_rpc_off.ensure((n_rpcs + 1) * 4);
+  s->d_rpc_ng.ensure((n_rpcs + 1) * 4);
+  s->d_rpc_res.ensure(n_rpcs * sizeof(yd_rpc_wait_result));
+  s->d_rpc_out.ensure(total * sizeof(yd_grant8));
+  s->d_out8.ensure(total * sizeof(yd_grant8));  // (a group's gathered window)
+  // the staged queue at its size class, so that the solve does not reallocate it
+  s->d_reqs.ensure(size_t(NextPow2(std::max<size_t>(hi - lo, 1), 1024)) * sizeof(yd_task_req));
+  const yd_rpc_wait* d_rpcs = s->d_rpcs.as<yd_rpc_wait>();
+  uint32_t* off = s->d_rpc_off.as<uint32_t>();
+  uint32_t* ng = s->d_rpc_ng.as<uint32_t>();
+  yd_rpc_wait_result* res = s->d_rpc_res.as<yd_rpc_wait_result>();
+  YD_CUDA_CHECK(cudaMemcpyAsync(s->d_rpcs.p, rpcs, n_rpcs * sizeof(yd_rpc_wait), cudaMemcpyHostToDevice, st));
+  yd::k_rpc_count<<<(n + 255) / 256, 256, 0, st>>>(d_rpcs, n, bound, off);
+  yd::k_scan_u32<<<1, 1024, 0, st>>>(off, n + 1, nullptr, 0, nullptr, 0);
+  uint32_t launches = 2;
+  if (hi > lo) {
+    yd::k_rpc_expand<<<(unsigned)((hi - lo + 255) / 256), 256, 0, st>>>(d_rpcs, n, bound, off, (uint32_t)lo, (uint32_t)hi,
+                                                                        s->d_reqs.as<yd_task_req>());
+    launches += 1;
+  }
+  YD_CUDA_CHECK(cudaGetLastError());
+  // the solve reads the staged queue on `st`, after the expansion
+  s->staged_n = hi - lo;
+  const uint64_t next0 = s->next_id;
+  if (group) {
+    if (ShardDecideWindow(s, now_ns, counts)) return (size_t)-1;
+  } else {
+    WaitImpl(s, now_ns, nullptr, nullptr, total, nullptr, nullptr, nullptr, true);
+  }
+  s->staged_n = 0;  // as the unpacked call leaves it: its queue went through the staging area
+  const uint64_t granted = s->next_id - next0;
+  const uint2* g8 = s->d_out8.as<uint2>();
+  yd::k_rpc_grants<<<(n + 255) / 256, 256, 0, st>>>(d_rpcs, n, off, g8, ng, res);
+  yd::k_scan_u32<<<1, 1024, 0, st>>>(ng, n + 1, nullptr, 0, nullptr, 0);
+  yd::k_rpc_report<<<(std::max(n, T) + 255) / 256, 256, 0, st>>>(n, T, off, g8, ng, res, s->d_rpc_out.as<uint2>());
+  launches += 3;
+  YD_CUDA_CHECK(cudaGetLastError());
+  YD_CUDA_CHECK(cudaMemcpyAsync(results, res, n_rpcs * sizeof(yd_rpc_wait_result), cudaMemcpyDeviceToHost, st));
+  if (granted) YD_CUDA_CHECK(cudaMemcpyAsync(grants_out, s->d_rpc_out.p, granted * sizeof(yd_grant8), cudaMemcpyDeviceToHost, st));
+  YD_CUDA_CHECK(cudaStreamSynchronize(st));
+  for (size_t i = 0; i != n_rpcs; ++i) {
+    if (results[i].reserved) {
+      fprintf(stderr, "ydsched: RPC %zu of a window has a grant outside its leading run\n", i);
+      abort();
+    }
+  }
+  if (!group) {
+    // the solve's stats, as the window's: its decisions, the kernels around the solve, and the window's records moved
+    // (the solve's scalars -- DynParams up, the counters down -- are not counted)
+    yd_solve_stats& stt = s->stats;
+    stt.decisions = total;
+    stt.kernel_launches += launches;
+    stt.h2d_bytes = n_rpcs * sizeof(yd_rpc_wait);
+    stt.d2h_bytes = n_rpcs * sizeof(yd_rpc_wait_result) + granted * sizeof(yd_grant8);
+  }
+  if (s->debug_env) {
+    fprintf(stderr, "ydsched: rpcs n_rpcs %zu decisions %zu range %zu %zu granted %llu expanded on device\n", n_rpcs, total,
+            lo, hi, (unsigned long long)granted);
+  }
+  return granted;
+}
+}  // namespace
+}  // extern "C++"
+
+size_t yd_wait_for_starting_task_rpcs_packed(yd_sched* s, int64_t now_ns, const yd_rpc_wait* rpcs, size_t n_rpcs,
+                                             yd_rpc_wait_result* results, yd_grant8* grants_out, size_t cap,
+                                             yd_packed_ids* ids) {
+  return RpcWindow(s, now_ns, rpcs, n_rpcs, results, grants_out, cap, ids, false);
+}
 
 // ---- compilation-cache bloom pre-filter (bloom.cuh) ------------------------------------------
 extern "C" {

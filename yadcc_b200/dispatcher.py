@@ -379,6 +379,25 @@ class TaskDispatcher:
         results[i] = (status, n_grants, first_grant) and grants is a GRANT_DTYPE array."""
         return self._rpcs_with(self._lib.yd_wait_for_starting_task_rpcs, rpcs, now)
 
+    def wait_for_starting_task_rpcs_packed(self, rpcs: np.ndarray, now: float = 0.0):
+        """wait_for_starting_task_rpcs with 8-byte grants (yd_wait_for_starting_task_rpcs_packed): returns (results,
+        GRANT8 array, PACKED_IDS record); grants8[k] has ordinal k, and `unpack_grants(grants8, ids)` gives the unpacked
+        call's grants."""
+        return self._rpcs_packed_with(self._optional_fn("yd_wait_for_starting_task_rpcs_packed"), rpcs, now)
+
+    def _rpcs_packed_with(self, fn, rpcs: np.ndarray, now: float):
+        assert rpcs.dtype == _abi.RPC_WAIT_DTYPE and rpcs.flags.c_contiguous
+        n = rpcs.shape[0]
+        cap = int(self._lib.yd_rpc_expanded_requests(self._h, rpcs.ctypes.data, n))  # counts clamped to what can be granted
+        results = np.zeros(n, dtype=_abi.RPC_RESULT_DTYPE)
+        grants8 = np.zeros(max(cap, 1), dtype=_abi.GRANT8_DTYPE)
+        ids = np.zeros(1, dtype=_abi.PACKED_IDS_DTYPE)
+        k = fn(self._h, _ns(now), rpcs.ctypes.data, n, results.ctypes.data, grants8.ctypes.data, cap, ids.ctypes.data)
+        if k == C.c_size_t(-1).value:
+            raise ValueError("the window was refused (grant buffer too small, staging memory, or a range-sharded group: "
+                             "capacities above 8192 per servant)")
+        return results, grants8[: int(k)], ids[0]
+
     def _rpcs_with(self, fn, rpcs: np.ndarray, now: float):
         assert rpcs.dtype == _abi.RPC_WAIT_DTYPE and rpcs.flags.c_contiguous
         n = rpcs.shape[0]

@@ -350,6 +350,13 @@ class RangeShardedDispatcher:
             return self.local.wait_for_starting_task_rpcs(rpcs, now)
         return self.local._rpcs_with(self.local._lib.yd_shard_wait_for_starting_task_rpcs, rpcs, now)
 
+    def wait_for_starting_task_rpcs_packed(self, rpcs: np.ndarray, now: float = 0.0):
+        """Replicated wait_for_starting_task_rpcs with 8-byte grants (yd_shard_wait_for_starting_task_rpcs_packed):
+        every rank gets the same (results, GRANT8 array, PACKED_IDS record) for the whole window."""
+        if not self.native:
+            return self.local.wait_for_starting_task_rpcs_packed(rpcs, now)
+        return self.local._rpcs_packed_with(self.local._lib.yd_shard_wait_for_starting_task_rpcs_packed, rpcs, now)
+
     # -- the pre-filtered solve (BASELINE configs[3]): each rank filters its own range, then the group decides the
     # concatenation of the offered ranges.  Both return this rank's (verdicts, hits, grants of its offered requests).
     def filter_and_wait_for_starting_new_tasks(self, reqs_local: np.ndarray, cache_keys=None, task_digests=None,
